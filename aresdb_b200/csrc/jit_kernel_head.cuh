@@ -35,7 +35,7 @@ struct JitParams {
   const uint8_t *wideValues[kJitMaxWide]; // 8/16-byte dimension columns read straight from global
   const uint8_t *wideNulls[kJitMaxWide];
   uint32_t consts[kJitMaxConsts];         // literal operands / mode-0 defaults (raw 32-bit cells)
-  unsigned long long magic[kJitMaxMagic]; // 2^64/d + 1 for literal divisors d > 0 (0: use the generic path)
+  unsigned long long magic[kJitMaxMagic]; // 2^64/d + 1 for literal divisors d >= 2 (0: use the generic path)
   unsigned long long measureIdentity;
   unsigned long long accNeutral;
   DevTable G;
@@ -141,7 +141,7 @@ __device__ __forceinline__ void ldrle(const RleColumn &R, uint32_t tile, const u
 }
 
 // x / d for a runtime-constant divisor as the high word of a 64x32-bit product (Lemire's fastdiv):
-// M = floor((2^64 - 1) / d) + 1; exact for every 32-bit x and d >= 1.  Two IMAD.WIDE.
+// M = floor((2^64 - 1) / d) + 1; exact for every 32-bit x and d >= 2 (for d = 1, M wraps to 0).  Two IMAD.WIDE.
 __device__ __forceinline__ uint32_t fastDivU32(uint32_t x, unsigned long long M) {
   const uint32_t carry = __umulhi((uint32_t)M, x);
   const unsigned long long hi = (unsigned long long)(uint32_t)(M >> 32) * x + carry;
