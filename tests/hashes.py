@@ -48,23 +48,35 @@ def _fmix64(k):
 
 
 def murmur3_128_lo(rows: np.ndarray) -> np.ndarray:
-    """rows: uint8[n, len], len <= 15 (tail only) -> low 64 bits of murmur3_x64_128(seed 0)."""
+    """rows: uint8[n, len], 0 < len <= 32 (the largest packed dimension row) -> low 64 bits of
+    murmur3_x64_128(seed 0).  16-byte body blocks, then the tail of len % 16 bytes."""
     n, ln = rows.shape
-    assert 0 < ln <= 15
-    pad = np.zeros((n, 16), np.uint8)
+    assert 0 < ln <= 32
+    blocks, tail = divmod(ln, 16)
+    pad = np.zeros((n, 32), np.uint8)
     pad[:, :ln] = rows
-    w = pad.view("<u8").reshape(n, 2)
+    w = pad.view("<u8").reshape(n, 4)
     c1, c2 = np.uint64(0x87c37b91114253d5), np.uint64(0x4cf5ad432745937f)
     with np.errstate(over="ignore"):
         h1 = np.zeros(n, np.uint64)
         h2 = np.zeros(n, np.uint64)
-        if ln > 8:
-            k2 = w[:, 1] * c2
+        for b in range(blocks):
+            k1 = _rotl64(w[:, 2 * b] * c1, 31) * c2
+            h1 ^= k1
+            h1 = _rotl64(h1, 27) + h2
+            h1 = h1 * np.uint64(5) + np.uint64(0x52dce729)
+            k2 = _rotl64(w[:, 2 * b + 1] * c2, 33) * c1
+            h2 ^= k2
+            h2 = _rotl64(h2, 31) + h1
+            h2 = h2 * np.uint64(5) + np.uint64(0x38495ab5)
+        if tail > 8:
+            k2 = w[:, 2 * blocks + 1] * c2
             k2 = _rotl64(k2, 33) * c1
             h2 ^= k2
-        k1 = w[:, 0] * c1
-        k1 = _rotl64(k1, 31) * c2
-        h1 ^= k1
+        if tail > 0:
+            k1 = w[:, 2 * blocks] * c1
+            k1 = _rotl64(k1, 31) * c2
+            h1 ^= k1
         h1 ^= np.uint64(ln)
         h2 ^= np.uint64(ln)
         h1 = h1 + h2

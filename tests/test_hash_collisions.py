@@ -81,6 +81,24 @@ def test_numpy_hashes_match_the_oracle():
         assert int(hashes.murmur3_128_lo(np.array([[v, 1]], np.uint8))[0]) == want
 
 
+def test_numpy_murmur3_128_matches_the_oracle_up_to_32_bytes():
+    """Every packed-row length the engine hashes (1..32 bytes: no body block, one and two 16-byte body blocks, each
+    tail length), against the oracle's byte-wise x64_128."""
+    dll = H.get_backend("oracle").lib.alg
+    dll.oracle_murmur3_128.restype = None
+    dll.oracle_murmur3_128.argtypes = [C.c_char_p, C.c_int, C.c_uint32, C.POINTER(C.c_uint64)]
+    rng = np.random.default_rng(6)
+    for ln in range(1, 33):
+        rows = rng.integers(0, 256, (40, ln), dtype=np.uint8)
+        rows[0] = 0
+        rows[1] = 255
+        got = hashes.murmur3_128_lo(rows)
+        for r, h in zip(rows, got):
+            out = (C.c_uint64 * 2)()
+            dll.oracle_murmur3_128(r.tobytes(), ln, 0, out)
+            assert out[0] == int(h), f"length {ln}"
+
+
 def collision_case():
     """Input rows in which two colliding pairs interleave with ordinary rows; returns everything the checks need."""
     (a1, b1), (a2, b2) = find_collisions32(2)
