@@ -275,6 +275,12 @@ __device__ __forceinline__ void keyInsert(uint64_t (&w)[KW], int byteOff, uint64
   }
 }
 
+// Group key of a packed dimension row: the row itself (KEY_PACKED), or the reference's hash of it.
+__device__ __forceinline__ unsigned long long rowKey(const uint64_t *w, uint8_t keyMode, uint8_t hashBits, int rowBytes) {
+  if (keyMode == KEY_PACKED) return w[0];
+  return hashBits == 64 ? murmur3_128_lo(w, rowBytes, 0) : (unsigned long long)murmur3_32(w, rowBytes, 0);
+}
+
 template <bool STAGED, bool WIDEKEY>
 __device__ __forceinline__ void processQuad(const DevPlan &P, const DevTable &G, const SmemTable &T, bool useSmem,
                                             bool allowClaim, const uint8_t *stage, uint32_t q, uint32_t row0,
@@ -390,7 +396,7 @@ __device__ __forceinline__ void processQuad(const DevPlan &P, const DevTable &G,
     unsigned long long key;
     const uint64_t *roww = nullptr;
     if constexpr (WIDEKEY) {
-      key = P.hashBits == 64 ? murmur3_128_lo(kw[r], P.rowBytes, 0) : (unsigned long long)murmur3_32(kw[r], P.rowBytes, 0);
+      key = rowKey(kw[r], KEY_HASHED, P.hashBits, P.rowBytes);
       if (P.hll == 1) key = (key & 0xFFFFFFFFFFFF0000ull) | (meas[r] & 0x3FFFu);
       roww = kw[r];
     } else {
@@ -533,32 +539,37 @@ fusedBatchKernel(const __grid_constant__ DevPlan P, const DevTable G) {
 // ---------------------------------------------------------------------------------------
 // merge of already-reduced rows, finalize
 // ---------------------------------------------------------------------------------------
+// Folds already-reduced row i (dimension block + measures) into the group table; `hll`: 0, 1 (entries), 2 (dense registers).
+__device__ __forceinline__ void foldRow(const uint8_t *__restrict__ block, const DimLayout &L, const uint8_t *__restrict__ measures,
+                                        uint32_t i, int width, AggOp op, uint8_t keyMode, uint8_t hashBits, int hll, const DevTable &G) {
+  uint64_t w[4];
+  packRow(block, L, i, w);
+  unsigned long long key = rowKey(w, keyMode, hashBits, L.rowBytes);
+  const uint64_t v = loadMeasure(measures, i, width);
+  if (hll == 2) { hllDenseUpdate(G, nullptr, key, keyMode == KEY_HASHED ? w : nullptr, (uint32_t)v); return; }
+  if (hll == 1) key = (key & 0xFFFFFFFFFFFF0000ull) | (v & 0x3FFFu);
+  globalUpdate(G, op, key, keyMode == KEY_HASHED ? w : nullptr, v);
+}
+
 __global__ void __launch_bounds__(256)
 mergeRowsKernel(const uint8_t *__restrict__ block, DimLayout L, const uint8_t *__restrict__ measures, int width,
                 AggOp op, int n, uint8_t keyMode, uint8_t hashBits, int hll, DevTable G) {
   const uint32_t stride = gridDim.x * blockDim.x;
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < (uint32_t)n; i += stride) {
-    uint64_t w[4];
-    packRow(block, L, i, w);
-    unsigned long long key = keyMode == KEY_PACKED ? w[0]
-                           : (hashBits == 64 ? murmur3_128_lo(w, L.rowBytes, 0) : (unsigned long long)murmur3_32(w, L.rowBytes, 0));
-    const uint64_t v = loadMeasure(measures, i, width);
-    if (hll == 2) { hllDenseUpdate(G, nullptr, key, keyMode == KEY_HASHED ? w : nullptr, (uint32_t)v); continue; }
-    if (hll == 1) key = (key & 0xFFFFFFFFFFFF0000ull) | (v & 0x3FFFu);
-    globalUpdate(G, op, key, keyMode == KEY_HASHED ? w : nullptr, v);
-  }
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < (uint32_t)n; i += stride)
+    foldRow(block, L, measures, i, width, op, keyMode, hashBits, hll, G);
 }
 
 // Exchange step of a sharded query, receiving side: all N gathered parts ([groups, status, rows | dimension block of
 // `L.capacity` rows | measures]) are folded by ONE launch; the row counts are read from the parts' headers on the
-// device, so the host never waits for them.  A part whose sender could not fit its rows raises counters[2].
+// device, so the host never waits for them.  A part whose sender could not fit its rows raises counters[2].  Parts carry no
+// HLL state (the export side refuses it).
 // `flags` != nullptr (exchange over peer memory, AggStateMergePartsWhenFlagged): the parts are written into this GPU's
 // memory by the PEERS' export kernels, each of which then stores `epoch` into flags[its rank] with release semantics at
 // system scope; every CTA waits for all numParts flags (acquire, system scope) before it reads a part.  The wait is
 // bounded (a peer that never arrives: counters[2], reported by finalize), so the kernel cannot hang the GPU.
 __global__ void __launch_bounds__(256)
 mergePartsKernel(const uint8_t *parts, int numParts, size_t partStride, size_t dimOff, size_t valOff, DimLayout L,
-                 int width, AggOp op, uint8_t keyMode, uint8_t hashBits, int hll, DevTable G, const uint32_t *flags, uint32_t epoch) {
+                 int width, AggOp op, uint8_t keyMode, uint8_t hashBits, DevTable G, const uint32_t *flags, uint32_t epoch) {
   const uint32_t stride = gridDim.x * blockDim.x;
   if (flags != nullptr) {
     __shared__ uint32_t sLate;
@@ -589,16 +600,8 @@ mergePartsKernel(const uint8_t *parts, int numParts, size_t partStride, size_t d
     }
     const uint32_t n = hdr[0];
     const uint8_t *block = part + dimOff, *measures = part + valOff;
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-      uint64_t w[4];
-      packRow(block, L, i, w);
-      unsigned long long key = keyMode == KEY_PACKED ? w[0]
-                             : (hashBits == 64 ? murmur3_128_lo(w, L.rowBytes, 0) : (unsigned long long)murmur3_32(w, L.rowBytes, 0));
-      const uint64_t v = loadMeasure(measures, i, width);
-      if (hll == 2) { hllDenseUpdate(G, nullptr, key, keyMode == KEY_HASHED ? w : nullptr, (uint32_t)v); continue; }
-      if (hll == 1) key = (key & 0xFFFFFFFFFFFF0000ull) | (v & 0x3FFFu);
-      globalUpdate(G, op, key, keyMode == KEY_HASHED ? w : nullptr, v);
-    }
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+      foldRow(block, L, measures, i, width, op, keyMode, hashBits, 0, G);
   }
 }
 
@@ -730,6 +733,23 @@ constexpr int kCmpThreads = 256;
 constexpr int kCmpItems = 8;
 constexpr int kCmpTile = kCmpThreads * kCmpItems;
 
+// Reference hash of the group whose table key is `key` (a packed key is its row; a hashed key already is the hash).
+__device__ __forceinline__ uint64_t groupHash(unsigned long long key, uint8_t keyMode, uint8_t hashBits, int rowBytes, uint64_t mask) {
+  uint64_t h = key;
+  if (keyMode == KEY_PACKED) {
+    const uint64_t w[4] = {key, 0, 0, 0};
+    h = rowKey(w, KEY_HASHED, hashBits, rowBytes);
+  }
+  return hashBits == 64 ? h & mask : h;
+}
+
+// Packed dimension row of the group in `slot`.
+__device__ __forceinline__ void slotRow(const DevTable &G, uint8_t keyMode, uint32_t slot, uint64_t (&w)[4]) {
+  if (keyMode == KEY_PACKED) { w[0] = G.keys[slot]; w[1] = w[2] = w[3] = 0; return; }
+#pragma unroll
+  for (int i = 0; i < 4; i++) w[i] = G.rows[(size_t)slot * 4 + i];
+}
+
 // Compacts occupied slots: slotOf[g] = slot index, hash[g] = reference hash of the group's row,
 // vals[g] = accumulator (tight `width`-byte elements).
 __global__ void __launch_bounds__(kCmpThreads)
@@ -763,16 +783,9 @@ compactGroupsKernel(DevTable G, size_t cap, uint8_t keyMode, uint8_t hashBits, u
   for (int k = 0; k < kCmpItems; k++) {
     if (!(mask & (1u << k))) continue;
     size_t i = base + k;
-    unsigned long long key = G.keys[i];
-    uint64_t h;
-    if (keyMode == KEY_PACKED) {
-      uint64_t w[4] = {key, 0, 0, 0};
-      h = hashBits == 64 ? murmur3_128_lo(w, rowBytes, 0) : (uint64_t)murmur3_32(w, rowBytes, 0);
-    } else {
-      h = key;
-    }
+    const uint64_t h = groupHash(G.keys[i], keyMode, hashBits, rowBytes, hashMask);
     slotOf[pos] = (uint32_t)i;
-    hash[pos] = hashBits == 64 ? h & hashMask : h;
+    hash[pos] = h;
     storeMeasure(vals, pos, width, G.acc[i]);
     pos++;
   }
@@ -785,16 +798,9 @@ gatherClaimedKernel(DevTable G, uint32_t n, uint8_t keyMode, uint8_t hashBits, u
   const uint32_t stride = gridDim.x * blockDim.x;
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
     const uint32_t slot = G.claimed[i];
-    const unsigned long long key = G.keys[slot];
-    uint64_t h;
-    if (keyMode == KEY_PACKED) {
-      uint64_t w[4] = {key, 0, 0, 0};
-      h = hashBits == 64 ? murmur3_128_lo(w, rowBytes, 0) : (uint64_t)murmur3_32(w, rowBytes, 0);
-    } else {
-      h = key;
-    }
+    const uint64_t h = groupHash(G.keys[slot], keyMode, hashBits, rowBytes, hashMask);
     slotOf[i] = slot;
-    hash[i] = hashBits == 64 ? h & hashMask : h;
+    hash[i] = h;
     storeMeasure(vals, i, width, G.acc[slot]);
   }
 }
@@ -804,14 +810,8 @@ emitGroupsKernel(DevTable G, uint8_t keyMode, const uint32_t *__restrict__ slotO
                  uint32_t g, uint8_t *__restrict__ outBlock, DimLayout L, uint32_t *__restrict__ outIndex) {
   const uint32_t stride = gridDim.x * blockDim.x;
   for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < g; s += stride) {
-    const uint32_t slot = slotOf[repIndex[s]];
     uint64_t w[4];
-    if (keyMode == KEY_PACKED) {
-      w[0] = G.keys[slot]; w[1] = w[2] = w[3] = 0;
-    } else {
-#pragma unroll
-      for (int i = 0; i < 4; i++) w[i] = G.rows[(size_t)slot * 4 + i];
-    }
+    slotRow(G, keyMode, slotOf[repIndex[s]], w);
     unpackRow(outBlock, L, s, w);
     if (outIndex) outIndex[s] = s;
   }
@@ -872,10 +872,7 @@ denseFoldKernel(unsigned long long *__restrict__ acc, DenseFold F, DevTable G) {
       for (int b = 0; b < F.width[k]; b++) rb[F.rowOff[k] + b] = (uint8_t)(val >> (8 * b));
       rb[F.nullOff[k]] = valid ? 1 : 0;
     }
-    unsigned long long key;
-    if (F.keyMode == KEY_PACKED) key = row[0];
-    else key = F.hashBits == 64 ? murmur3_128_lo(row, F.rowBytes, 0) : (unsigned long long)murmur3_32(row, F.rowBytes, 0);
-    globalUpdate(G, (AggOp)F.op, key, F.keyMode == KEY_PACKED ? nullptr : row, v);
+    globalUpdate(G, (AggOp)F.op, rowKey(row, F.keyMode, F.hashBits, F.rowBytes), F.keyMode == KEY_PACKED ? nullptr : row, v);
   }
 }
 
@@ -913,6 +910,18 @@ struct SmallFinalizeArgs {
   uint8_t keyMode, hashBits, op, plusZero, ordered;
 };
 
+// The exchange form: the n claimed slots as they are, in claim order, no sort and no merge.
+__device__ __forceinline__ void exportClaimed(const SmallFinalizeArgs &A, uint32_t n, uint32_t gtid) {
+  for (uint32_t i = gtid; i < n; i += kFinThreads) {
+    const uint32_t slot = A.G.claimed[i];
+    uint64_t w[4];
+    slotRow(A.G, A.keyMode, slot, w);
+    unpackRow(A.outBlock, A.L, i, w);
+    storeMeasure(A.outValues, i, A.width, A.G.acc[slot]);
+    if (A.outIndex) A.outIndex[i] = i;
+  }
+}
+
 __global__ void __cluster_dims__(kFinCtas, 1, 1) __launch_bounds__(1024) finalizeSmallKernel(const __grid_constant__ SmallFinalizeArgs A) {
   __shared__ uint32_t off[kSmallBuckets + 1];
   __shared__ uint32_t sWarp[1024 / 32 + 1];
@@ -935,22 +944,8 @@ __global__ void __cluster_dims__(kFinCtas, 1, 1) __launch_bounds__(1024) finaliz
     if (gtid == 0) publish(0, status, n);
     return;
   }
-  auto rowOf = [&](uint32_t slot, uint64_t (&w)[4]) {
-    if (A.keyMode == KEY_PACKED) { w[0] = G.keys[slot]; w[1] = w[2] = w[3] = 0; }
-    else {
-#pragma unroll
-      for (int i = 0; i < 4; i++) w[i] = G.rows[(size_t)slot * 4 + i];
-    }
-  };
   if (!A.ordered) {
-    for (uint32_t i = gtid; i < n; i += kFinThreads) {
-      const uint32_t slot = G.claimed[i];
-      uint64_t w[4];
-      rowOf(slot, w);
-      unpackRow(A.outBlock, A.L, i, w);
-      storeMeasure(A.outValues, i, A.width, G.acc[slot]);
-      if (A.outIndex) A.outIndex[i] = i;
-    }
+    exportClaimed(A, n, gtid);
     if (gtid == 0) publish(n, SF_OK, n);
     return;
   }
@@ -960,14 +955,7 @@ __global__ void __cluster_dims__(kFinCtas, 1, 1) __launch_bounds__(1024) finaliz
   cluster.sync();
   // 1. reference hash of every group's row; histogram of the top hash bits
   for (uint32_t i = gtid; i < n; i += kFinThreads) {
-    const unsigned long long key = G.keys[G.claimed[i]];
-    uint64_t h;
-    if (A.keyMode == KEY_PACKED) {
-      uint64_t w[4] = {key, 0, 0, 0};
-      h = A.hashBits == 64 ? murmur3_128_lo(w, A.rowBytes, 0) & A.hashMask : (uint64_t)murmur3_32(w, A.rowBytes, 0);
-    } else {
-      h = A.hashBits == 64 ? key & A.hashMask : key;
-    }
+    const uint64_t h = groupHash(G.keys[G.claimed[i]], A.keyMode, A.hashBits, A.rowBytes, A.hashMask);
     A.hashA[i] = h;
     atomicAdd(&cnt[(uint32_t)(h >> shift) & (kSmallBuckets - 1)], 1u);
   }
@@ -1041,7 +1029,7 @@ __global__ void __cluster_dims__(kFinCtas, 1, 1) __launch_bounds__(1024) finaliz
       else acc = __float_as_uint(__uint_as_float((uint32_t)acc) + 0.0f);
     }
     uint64_t w[4];
-    rowOf(slot, w);
+    slotRow(G, A.keyMode, slot, w);
     unpackRow(A.outBlock, A.L, pos, w);
     storeMeasure(A.outValues, pos, A.width, acc);
     if (A.outHash) A.outHash[pos] = h;
@@ -1074,19 +1062,7 @@ __global__ void __cluster_dims__(kFinCtas, 1, 1) __launch_bounds__(1024) exportT
   if (G.counters[1]) status = SF_TABLE_OVERFLOW;
   else if (G.counters[3] || G.counters[4]) status = SF_UNSETTLED;
   else if (n > (uint32_t)A.outCapacity) status = SF_OUTPUT_TOO_SMALL;
-  if (status == SF_OK) {
-    for (uint32_t i = gtid; i < n; i += kFinThreads) {
-      const uint32_t slot = G.claimed[i];
-      uint64_t w[4];
-      if (A.keyMode == KEY_PACKED) { w[0] = G.keys[slot]; w[1] = w[2] = w[3] = 0; }
-      else {
-#pragma unroll
-        for (int k = 0; k < 4; k++) w[k] = G.rows[(size_t)slot * 4 + k];
-      }
-      unpackRow(A.outBlock, A.L, i, w);
-      storeMeasure(A.outValues, i, A.width, G.acc[slot]);
-    }
-  }
+  if (status == SF_OK) exportClaimed(A, n, gtid);
   if (gtid == 0) { A.resultDev[0] = status == SF_OK ? n : 0u; A.resultDev[1] = status; A.resultDev[2] = n; }
   cluster.sync();   // the local part is complete (and visible to the cluster)
   // the part travels as it lies: header, the used prefix of every section would save bytes, but a part is 0.5 MB and the
@@ -1153,6 +1129,16 @@ struct AggState {
 
 constexpr size_t kHllDenseSlots = 8192;
 
+// DevPlan::hll and mergeRowsKernel's `hll`: 0 no HLL, 1 (group, register) entries, 2 dense register arrays
+static uint8_t hllMode(const AggState *st) { return st->hll ? (st->hllDense ? 2 : 1) : 0; }
+
+static void *deviceAllocOrThrow(size_t bytes) {
+  void *mem = nullptr;
+  CGoCallResHandle h = deviceMalloc(&mem, bytes);
+  if (h.pStrErr) { std::string m(h.pStrErr); free((void *)h.pStrErr); throw EngineError(m); }
+  return mem;
+}
+
 static uint64_t neutralOf(AggOp op) {
   switch (op) {
     case OP_SUM_F32: return 0x80000000ull;                // -0.0f: (-0) + x == x for every x
@@ -1186,9 +1172,7 @@ static void allocTable(AggState *st, size_t cap, cudaStream_t s) {
   const size_t progressBytes = ((size_t)(kProgressTail + 1) * 4 + 255) / 256 * 256;
   const size_t spillBytes = (size_t)kSpillCap * sizeof(SpillEntry);
   size_t bytes = cap * 16 + (rows ? cap * 32 : 0) + 256 + ctaAccBytes + regBytes + claimedBytes + smallBytes + progressBytes + spillBytes;
-  void *mem = nullptr;
-  CGoCallResHandle h = deviceMalloc(&mem, bytes);
-  if (h.pStrErr) { std::string m(h.pStrErr); free((void *)h.pStrErr); throw EngineError(m); }
+  void *mem = deviceAllocOrThrow(bytes);
   st->mem = mem;
   st->capacity = cap;
   uint8_t *p = static_cast<uint8_t *>(mem);
@@ -1488,7 +1472,7 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P) {
   }
   P.measWidth = (uint8_t)st->measWidth;
   P.measClass = st->measClass;
-  P.hll = st->hll ? (st->hllDense ? 2 : 1) : 0;
+  P.hll = hllMode(st);
   P.denseSlots = st->hllDense ? (uint32_t)st->capacity : 0;
   const int agg = st->spec.AggFunc;
   P.skipCount = !((agg >= AGGR_SUM_UNSIGNED && agg <= AGGR_SUM_FLOAT) || agg == AGGR_AVG_FLOAT);
@@ -1574,10 +1558,6 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups, bool allowDense 
   P.denseGlobal = 0;
   if (allowDense) jitAnalyzeDense(P, P.bypassOk != 0);
   else P.denseNd = 0;
-  if (const char *e = getenv("ARESDB_B200_SMEM_SLOTS")) {  // tuning / experiments
-    uint32_t v = (uint32_t)atoi(e);
-    if (v >= 256 && v <= 8192 && (v & (v - 1)) == 0) slots = v;
-  }
   auto stageBytesFor = [&](uint32_t tr) {
     size_t stage = 0;
     for (int c = 0; c < P.ncols; c++) {
@@ -1592,14 +1572,11 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups, bool allowDense 
   };
   uint32_t tileRows = 0, stages = 0;
   if (canStage && rowBits > 0) {
-    uint32_t forceTile = 0;
-    if (const char *e = getenv("ARESDB_B200_TILE_ROWS")) forceTile = (uint32_t)atoi(e);  // tuning / experiments
     if (P.denseNd != 0) {
       // Dense slots cost 9 bytes each (flag + 8-byte accumulator).  Give the ring as many stages as possible
       // and the slots the rest: the capacity (part of the kernel text) then depends on the stage layout only,
       // not on the batch's ranges.
       for (uint32_t tr : {3968u, 1920u, 896u}) {
-        if (forceTile && tr != forceTile) continue;
         for (uint32_t n = kMaxStages; n >= 2 && !tileRows; n--) {
           const size_t need = 128 + n * stageBytesFor(tr);
           if (need >= (size_t)kSmemBudget) continue;
@@ -1614,7 +1591,6 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups, bool allowDense 
       if (!tileRows && !P.hll && P.neutralSafe && P.denseTotal <= kGlobalDenseMaxSlots) {
         // more slots than a CTA holds: one accumulator array in global memory for the whole grid; shared memory is all ring
         for (uint32_t tr : {3968u, 1920u, 896u}) {
-          if (forceTile && tr != forceTile) continue;
           const uint32_t n = (uint32_t)(((size_t)kSmemBudget - 128 - 256) / stageBytesFor(tr));
           if (n >= 2) {
             tileRows = tr; stages = n > (uint32_t)kMaxStages ? kMaxStages : n; slots = 16; P.denseGlobal = 1;
@@ -1622,7 +1598,6 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups, bool allowDense 
             // replicate the slot array until it has about that many
             uint32_t reps = 1;
             while (reps < 8 && (uint64_t)P.denseTotal * reps * 2 <= kGlobalDenseMaxSlots && (uint64_t)P.denseTotal * reps < (1u << 20)) reps *= 2;
-            if (const char *e = getenv("ARESDB_B200_GLOBAL_REPS")) { const int v = atoi(e); if (v >= 1 && v <= 8 && (v & (v - 1)) == 0 && (uint64_t)P.denseTotal * v <= kGlobalDenseMaxSlots) reps = (uint32_t)v; }
             P.denseGlobalReps = (uint8_t)reps;
             break;
           }
@@ -1631,20 +1606,10 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups, bool allowDense 
       if (!tileRows) P.denseNd = 0;   // no layout holds the slots: hash table
     }
     if (!tileRows) {
-      // compacted-index form (survivors of the filters gathered per tile before the expensive part)
-      P.compact = 0;
-      if (allowDense && P.denseNd == 0 && jitAvailable() && planCompactable(P)) {
-        // (opt-in only: on cfg4 HLL without zone maps the kernel is bound by the latency of its directory / register
-        // accesses, and the barrier of the compaction cost more than the instructions it saves when it was measured)
-        const char *e = getenv("ARESDB_B200_COMPACT");
-        P.compact = e ? (e[0] == '1') : 0;
-      }
-      if (P.partition) P.compact = 0;
       for (uint32_t sl : {slots, slots / 2, slots / 4}) {
         if (P.partition && sl != 8192) break;      // the tile buffer of the partitioned form IS the 64 KB table region
         for (uint32_t tr : {3968u, 1920u, 896u}) {  // 128 rows x (31 | 15 | 7) consumer warps
-          if (forceTile && tr != forceTile) continue;
-          size_t avail = (size_t)kSmemBudget - 128 - (size_t)sl * 8 - (P.compact ? kCompactListBytes : 0u) - (P.partition ? kPartitionExtraBytes : 0u);
+          size_t avail = (size_t)kSmemBudget - 128 - (size_t)sl * 8 - (P.partition ? kPartitionExtraBytes : 0u);
           uint32_t n = (uint32_t)(avail / stageBytesFor(tr));
           if (n >= 2) { tileRows = tr; stages = n > (uint32_t)kMaxStages ? kMaxStages : n; break; }
         }
@@ -1693,9 +1658,9 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups, bool allowDense 
   P.stageBytes = (uint32_t)stageBytes;
   P.smemSlots = slots;
   P.tableBytes = P.denseNd != 0 ? (slots * (P.hll ? 4 : P.denseFx ? 12 : 9) + 127) / 128 * 128 : slots * 8;
-  if (P.denseNd != 0 || !P.staged) { P.compact = 0; P.partition = 0; }
+  if (P.denseNd != 0 || !P.staged) P.partition = 0;
   if (P.partition && (slots != 8192 || P.tileRows > 4096)) P.partition = 0;
-  return 128 + (size_t)P.tableBytes + (P.compact ? kCompactListBytes : 0u) + (P.partition ? kPartitionExtraBytes : 0u) + stageBytes * P.numStages;
+  return 128 + (size_t)P.tableBytes + (P.partition ? kPartitionExtraBytes : 0u) + stageBytes * P.numStages;
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1744,7 +1709,16 @@ partitionAggregateKernel(const uint4 *__restrict__ entries, const uint32_t *__re
 }
 
 struct TableCounters { uint32_t occupied, overflow, truncated, stop, spilled, spillOverflow; };
-static void checkOverflow(AggState *st, const uint32_t counters[2]);
+
+// Throws when the table's overflow counter is set.
+static void checkOverflow(const AggState *st, uint32_t overflow) {
+  if (!overflow) return;
+  if (st->hllDense)
+    throw EngineError("dense HLL state: more than " + std::to_string(kHllDenseMaxGroups) +
+                      " dimension groups; recreate the AggState with AggSpec.ExpectedGroups > 4096 (entry mode) and replay the batches");
+  throw EngineError("group table overflow: more than " + std::to_string(st->capacity) +
+                    " slots needed; recreate the AggState with a larger AggSpec.ExpectedGroups and replay the batches");
+}
 
 static TableCounters readCounters(AggState *st, cudaStream_t s) {
   TableCounters c;
@@ -1792,7 +1766,7 @@ static void settleTable(AggState *st, cudaStream_t s) {
   if (c.spillOverflow)
     throw EngineError("group table: more than " + std::to_string(kSpillCap) + " rows of new groups arrived from direct-indexed batches while the "
                       "table was full (a zone map far off the data); recreate the AggState with a larger AggSpec.ExpectedGroups and replay");
-  if (c.overflow) checkOverflow(st, &c.occupied);
+  checkOverflow(st, c.overflow);
   if (c.stop && st->unchecked > 0) {
     const uint32_t n = st->unchecked;
     st->unchecked = 0;
@@ -1837,11 +1811,9 @@ static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
   //    uncompressed column (values / null bitmap of its runs), no copy;
   //  * every other RLE column is a FIRST-CLASS input of the specialised kernel: decoded from its runs inside the tile loop
   //    (jit_kernel_head.cuh ldrle) with a per-tile run hint computed below — HBM sees the runs, not the rows;
-  //  * without NVRTC (or with ARESDB_B200_EXPAND_RLE=1) the column is expanded once per batch for the interpreter.
+  //  * without NVRTC the column is expanded once per batch for the interpreter.
   std::vector<std::unique_ptr<Scratch>> expanded;
-  static const bool forceExpand = [] { const char *e = getenv("ARESDB_B200_EXPAND_RLE"); return e && e[0] == '1'; }();
-  static const bool keepPositional = [] { const char *e = getenv("ARESDB_B200_EXPAND_RLE"); return e && e[0] == '0'; }();
-  if (bp.NumRows >= 1024 && !keepPositional) {
+  if (bp.NumRows >= 1024) {
     const uint32_t n = bp.NumRows;
     // (the tile loop is driven by the TMA ring: at least one plain column must be staged for the RLE columns to ride along)
     int stageable = 0;
@@ -1851,7 +1823,7 @@ static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
       if (col.used && col.in.mode == 3 && col.width <= 4 && bp.BaseCounts != nullptr &&
           reinterpret_cast<const uint32_t *>(col.in.base) == bp.BaseCounts && col.in.length >= n) stageable++;
     }
-    const bool firstClass = jitAvailable() && !forceExpand && stageable > 0;
+    const bool firstClass = jitAvailable() && stageable > 0;
     int nrle = 0;
     for (int c = 0; c < P.ncols; c++) {
       DevColumn &col = P.cols[c];
@@ -1957,10 +1929,7 @@ static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
   int grid = gridFor();
   if (P.denseGlobal) {
     if (!st->denseAcc) {   // first use: 16 MB of accumulators at the neutral element (denseFoldKernel leaves them so)
-      void *mem = nullptr;
-      CGoCallResHandle h = deviceMalloc(&mem, (size_t)kGlobalDenseMaxSlots * sizeof(unsigned long long));
-      if (h.pStrErr) { std::string m(h.pStrErr); free((void *)h.pStrErr); throw EngineError(m); }
-      st->denseAcc = static_cast<unsigned long long *>(mem);
+      st->denseAcc = static_cast<unsigned long long *>(deviceAllocOrThrow((size_t)kGlobalDenseMaxSlots * sizeof(unsigned long long)));
       fillTableKernel<<<smCount() * 8, 256, 0, s>>>(st->denseAcc, st->denseAcc, kGlobalDenseMaxSlots, st->accNeutral);
       checkLastError("denseAcc fill");
     }
@@ -1977,7 +1946,7 @@ static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
         checkLastError("partitionAggregate");
         const TableCounters c = readCounters(st, s);
         st->everChecked = true;
-        if (c.overflow) checkOverflow(st, &c.occupied);
+        checkOverflow(st, c.overflow);
         if (c.stop || c.spilled) settleTable(st, s);
         return;
       }
@@ -2023,7 +1992,7 @@ static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
     }
     const TableCounters c = readCounters(st, s);
     st->everChecked = true;
-    if (c.overflow) checkOverflow(st, &c.occupied);
+    checkOverflow(st, c.overflow);
     if (!c.stop && !c.spilled) { st->unchecked = 0; return; }
     if (c.stop && st->unchecked > 0) settleTable(st, s);   // raises: earlier unwatched batches stopped as well
     const bool stopped = c.stop != 0;
@@ -2043,17 +2012,8 @@ static void mergeRows(AggState *st, const DimensionVector &in, const uint8_t *va
   int blocks = divUp(length, 256);
   if (blocks > smCount() * 8) blocks = smCount() * 8;
   mergeRowsKernel<<<blocks, 256, 0, s>>>(in.DimValues, L, values, st->measWidth, st->op, length, st->keyMode,
-                                        (uint8_t)st->hashBits, st->hll ? (st->hllDense ? 2 : 1) : 0, st->table);
+                                        (uint8_t)st->hashBits, hllMode(st), st->table);
   checkLastError("AggStateMerge");
-}
-
-static void checkOverflow(AggState *st, const uint32_t counters[2]) {
-  if (counters[1] && st->hllDense)
-    throw EngineError("dense HLL state: more than " + std::to_string(kHllDenseMaxGroups) +
-                      " dimension groups; recreate the AggState with AggSpec.ExpectedGroups > 4096 (entry mode) and replay the batches");
-  if (counters[1])
-    throw EngineError("group table overflow: more than " + std::to_string(st->capacity) +
-                      " slots needed; recreate the AggState with a larger AggSpec.ExpectedGroups and replay the batches");
 }
 
 static int64_t groupCount(AggState *st, cudaStream_t s) {
@@ -2062,7 +2022,7 @@ static int64_t groupCount(AggState *st, cudaStream_t s) {
     settleTable(st, s);
     c = readCounters(st, s);
   }
-  checkOverflow(st, &c.occupied);
+  checkOverflow(st, c.overflow);
   return c.occupied;
 }
 
@@ -2074,30 +2034,48 @@ struct DenseCarried {
   Scratch block, hash, values, index;
 };
 
-static void denseCarried(AggState *st, cudaStream_t s, DenseCarried &out, bool countOnly) {
+// The claimed groups of a dense HLL state in the order of the reference hash of their dim row: the d-th group is in
+// directory slot slotOf[order[d]], hash[d] is its hash.
+struct DenseGroups {
+  int n = 0;
+  Scratch slotOf, hash, order;
+};
+
+static void denseGroups(AggState *st, cudaStream_t s, DenseGroups &out) {
   uint32_t c[2];
   ARES_CUDA(cudaMemcpyAsync(c, st->table.counters, sizeof(c), cudaMemcpyDeviceToHost, s));
   ARES_CUDA(cudaStreamSynchronize(s));
-  checkOverflow(st, c);
+  checkOverflow(st, c[1]);
   const int n = (int)c[0];
-  out.groups = n;
-  out.entries = 0;
+  out.n = n;
   if (n == 0) return;
-  // groups in the order of the reference hash of their dim row
   const int tiles = divUp((int64_t)st->capacity, kCmpTile);
   Scratch state(scanStateBytes(tiles) + sizeof(uint32_t), s);
   ARES_CUDA(cudaMemsetAsync(state.ptr, 0, state.bytes, s));
   ScanTileState sst = makeScanState(state.ptr, tiles);
   uint32_t *dCount = reinterpret_cast<uint32_t *>(static_cast<uint8_t *>(state.ptr) + scanStateBytes(tiles));
-  Scratch slotOf(sizeof(uint32_t) * (size_t)n, s), hash(sizeof(uint64_t) * (size_t)n, s), vals(sizeof(uint32_t) * (size_t)n, s);
+  out.slotOf.reset(sizeof(uint32_t) * (size_t)n, s);
+  out.hash.reset(sizeof(uint64_t) * (size_t)n, s);
+  out.order.reset(sizeof(uint32_t) * (size_t)n, s);
+  Scratch vals(sizeof(uint32_t) * (size_t)n, s);
   compactGroupsKernel<<<tiles, kCmpThreads, 0, s>>>(st->table, st->capacity, st->keyMode, 64, ~0ull, st->rowLayout.rowBytes, 4, sst,
-                                                   slotOf.as<uint32_t>(), hash.as<uint64_t>(), vals.as<uint8_t>(), dCount);
+                                                   out.slotOf.as<uint32_t>(), out.hash.as<uint64_t>(), vals.as<uint8_t>(), dCount);
   checkLastError("compactGroups");
-  Scratch order(sizeof(uint32_t) * (size_t)n, s), tmpK(sizeof(uint64_t) * (size_t)n, s), tmpV(sizeof(uint32_t) * (size_t)n, s);
-  iotaKernel<<<divUp(n, 256), 256, 0, s>>>(order.as<uint32_t>(), n);
-  sortKeyIndexPairs(hash.as<uint64_t>(), order.as<uint32_t>(), tmpK.as<uint64_t>(), tmpV.as<uint32_t>(), n, 64, s);
+  Scratch tmpK(sizeof(uint64_t) * (size_t)n, s), tmpV(sizeof(uint32_t) * (size_t)n, s);
+  iotaKernel<<<divUp(n, 256), 256, 0, s>>>(out.order.as<uint32_t>(), n);
+  sortKeyIndexPairs(out.hash.as<uint64_t>(), out.order.as<uint32_t>(), tmpK.as<uint64_t>(), tmpV.as<uint32_t>(), n, 64, s);
+}
+
+static void denseCarried(AggState *st, cudaStream_t s, DenseCarried &out, bool countOnly) {
+  DenseGroups dg;
+  denseGroups(st, s, dg);
+  const int n = dg.n;
+  out.groups = n;
+  out.entries = 0;
+  if (n == 0) return;
+  uint32_t *slotOf = dg.slotOf.as<uint32_t>(), *order = dg.order.as<uint32_t>();
   Scratch counts(sizeof(uint32_t) * (size_t)n, s), offsets(sizeof(uint32_t) * ((size_t)n + 1), s);
-  hllDenseCountKernel<<<n, 256, 0, s>>>(st->table.regs, st->table.acc, slotOf.as<uint32_t>(), order.as<uint32_t>(), counts.as<uint32_t>());
+  hllDenseCountKernel<<<n, 256, 0, s>>>(st->table.regs, st->table.acc, slotOf, order, counts.as<uint32_t>());
   checkLastError("hllDenseCount");
   hllDenseOffsetsKernel<<<1, 1024, 0, s>>>(counts.as<uint32_t>(), n, offsets.as<uint32_t>());
   checkLastError("hllDenseOffsets");
@@ -2111,12 +2089,10 @@ static void denseCarried(AggState *st, cudaStream_t s, DenseCarried &out, bool c
   out.values.reset(sizeof(uint32_t) * (size_t)total, s);
   out.index.reset(sizeof(uint32_t) * (size_t)total, s);
   DimLayout L = makeDimLayout(st->spec.NumDimsPerDimWidth, n);
-  emitGroupsKernel<<<divUp(n, 256), 256, 0, s>>>(st->table, st->keyMode, slotOf.as<uint32_t>(), order.as<uint32_t>(), (uint32_t)n,
-                                                 out.block.as<uint8_t>(), L, nullptr);
+  emitGroupsKernel<<<divUp(n, 256), 256, 0, s>>>(st->table, st->keyMode, slotOf, order, (uint32_t)n, out.block.as<uint8_t>(), L, nullptr);
   checkLastError("emitGroups");
-  hllDenseEmitKernel<<<n, 256, 0, s>>>(st->table.regs, st->table.acc, slotOf.as<uint32_t>(), order.as<uint32_t>(), hash.as<uint64_t>(),
-                                       offsets.as<uint32_t>(), out.hash.as<uint64_t>(), out.values.as<uint32_t>(),
-                                       out.index.as<uint32_t>());
+  hllDenseEmitKernel<<<n, 256, 0, s>>>(st->table.regs, st->table.acc, slotOf, order, dg.hash.as<uint64_t>(), offsets.as<uint32_t>(),
+                                       out.hash.as<uint64_t>(), out.values.as<uint32_t>(), out.index.as<uint32_t>());
   checkLastError("hllDenseEmit");
   ARES_CUDA(cudaStreamSynchronize(s));  // the locals above are released in stream order; keep it simple
 }
@@ -2124,28 +2100,14 @@ static void denseCarried(AggState *st, cudaStream_t s, DenseCarried &out, bool c
 // Dense HLL state -> the final outputs of AggStateFinalizeHLL, straight from the register arrays.
 static int64_t denseVectors(AggState *st, cudaStream_t s, uint8_t **dimValuesPtr, uint8_t **hllVectorPtr, size_t *hllVectorSizePtr,
                             uint16_t **hllDimRegIDCountPtr) {
-  uint32_t c[2];
-  ARES_CUDA(cudaMemcpyAsync(c, st->table.counters, sizeof(c), cudaMemcpyDeviceToHost, s));
-  ARES_CUDA(cudaStreamSynchronize(s));
-  checkOverflow(st, c);
-  const int n = (int)c[0];
+  DenseGroups dg;
+  denseGroups(st, s, dg);
+  const int n = dg.n;
   if (n == 0) return 0;
-  // groups in the order of the reference hash of their dim row
-  const int tiles = divUp((int64_t)st->capacity, kCmpTile);
-  Scratch state(scanStateBytes(tiles) + sizeof(uint32_t), s);
-  ARES_CUDA(cudaMemsetAsync(state.ptr, 0, state.bytes, s));
-  ScanTileState sst = makeScanState(state.ptr, tiles);
-  uint32_t *dCount = reinterpret_cast<uint32_t *>(static_cast<uint8_t *>(state.ptr) + scanStateBytes(tiles));
-  Scratch slotOf(sizeof(uint32_t) * (size_t)n, s), hash(sizeof(uint64_t) * (size_t)n, s), vals(sizeof(uint32_t) * (size_t)n, s);
-  compactGroupsKernel<<<tiles, kCmpThreads, 0, s>>>(st->table, st->capacity, st->keyMode, 64, ~0ull, st->rowLayout.rowBytes, 4, sst,
-                                                   slotOf.as<uint32_t>(), hash.as<uint64_t>(), vals.as<uint8_t>(), dCount);
-  checkLastError("compactGroups");
-  Scratch order(sizeof(uint32_t) * (size_t)n, s), tmpK(sizeof(uint64_t) * (size_t)n, s), tmpV(sizeof(uint32_t) * (size_t)n, s);
-  iotaKernel<<<divUp(n, 256), 256, 0, s>>>(order.as<uint32_t>(), n);
-  sortKeyIndexPairs(hash.as<uint64_t>(), order.as<uint32_t>(), tmpK.as<uint64_t>(), tmpV.as<uint32_t>(), n, 64, s);
+  uint32_t *slotOf = dg.slotOf.as<uint32_t>(), *order = dg.order.as<uint32_t>();
   Scratch counts(sizeof(uint32_t) * (size_t)n, s), outIdx(sizeof(uint32_t) * (size_t)n, s), byteOff(sizeof(uint32_t) * (size_t)n, s);
   Scratch rowsOf(sizeof(uint32_t) * (size_t)n, s), totalsDev(sizeof(unsigned long long) * 2, s);
-  hllDenseCountKernel<<<n, 256, 0, s>>>(st->table.regs, st->table.acc, slotOf.as<uint32_t>(), order.as<uint32_t>(), counts.as<uint32_t>());
+  hllDenseCountKernel<<<n, 256, 0, s>>>(st->table.regs, st->table.acc, slotOf, order, counts.as<uint32_t>());
   checkLastError("hllDenseCount");
   hllVectorLayoutKernel<<<1, 1024, 0, s>>>(counts.as<uint32_t>(), n, outIdx.as<uint32_t>(), byteOff.as<uint32_t>(), rowsOf.as<uint32_t>(),
                                           totalsDev.as<unsigned long long>());
@@ -2153,30 +2115,24 @@ static int64_t denseVectors(AggState *st, cudaStream_t s, uint8_t **dimValuesPtr
   // the groups' dim rows in hash order (the groups with registers are picked out of it below)
   Scratch blockAll((size_t)st->rowLayout.rowBytes * n, s);
   DimLayout Lin = makeDimLayout(st->spec.NumDimsPerDimWidth, n);
-  emitGroupsKernel<<<divUp(n, 256), 256, 0, s>>>(st->table, st->keyMode, slotOf.as<uint32_t>(), order.as<uint32_t>(), (uint32_t)n,
-                                                 blockAll.as<uint8_t>(), Lin, nullptr);
+  emitGroupsKernel<<<divUp(n, 256), 256, 0, s>>>(st->table, st->keyMode, slotOf, order, (uint32_t)n, blockAll.as<uint8_t>(), Lin, nullptr);
   checkLastError("emitGroups");
   unsigned long long totals[2] = {0, 0};
   ARES_CUDA(cudaMemcpyAsync(totals, totalsDev.ptr, sizeof(totals), cudaMemcpyDeviceToHost, s));
   ARES_CUDA(cudaStreamSynchronize(s));
   const int dims = (int)totals[0];
   if (dims == 0) return 0;
-  void *vec = nullptr, *cnt = nullptr, *out = nullptr;
-  auto fail = [&](CGoCallResHandle h) {
-    std::string m(h.pStrErr); free((void *)h.pStrErr);
-    if (vec) deviceFree(vec);
+  void *vec = deviceAllocOrThrow((size_t)totals[1]), *cnt = nullptr, *out = nullptr;
+  try {
+    cnt = deviceAllocOrThrow(sizeof(uint16_t) * (size_t)dims);
+    out = deviceAllocOrThrow((size_t)st->rowLayout.rowBytes * dims);
+  } catch (...) {
+    deviceFree(vec);
     if (cnt) deviceFree(cnt);
-    throw EngineError(m);
-  };
-  CGoCallResHandle h = deviceMalloc(&vec, (size_t)totals[1]);
-  if (h.pStrErr) fail(h);
-  h = deviceMalloc(&cnt, sizeof(uint16_t) * (size_t)dims);
-  if (h.pStrErr) fail(h);
-  h = deviceMalloc(&out, (size_t)st->rowLayout.rowBytes * dims);
-  if (h.pStrErr) fail(h);
-  hllVectorEmitKernel<<<n, 256, 0, s>>>(st->table.regs, st->table.acc, slotOf.as<uint32_t>(), order.as<uint32_t>(), counts.as<uint32_t>(),
-                                        outIdx.as<uint32_t>(), byteOff.as<uint32_t>(), static_cast<uint8_t *>(vec),
-                                        static_cast<uint16_t *>(cnt));
+    throw;
+  }
+  hllVectorEmitKernel<<<n, 256, 0, s>>>(st->table.regs, st->table.acc, slotOf, order, counts.as<uint32_t>(), outIdx.as<uint32_t>(),
+                                        byteOff.as<uint32_t>(), static_cast<uint8_t *>(vec), static_cast<uint16_t *>(cnt));
   checkLastError("hllVectorEmit");
   DimLayout Lout = makeDimLayout(st->spec.NumDimsPerDimWidth, dims);
   gatherDims(blockAll.as<uint8_t>(), Lin, rowsOf.as<uint32_t>(), dims, static_cast<uint8_t *>(out), Lout, s);
@@ -2186,6 +2142,19 @@ static int64_t denseVectors(AggState *st, cudaStream_t s, uint8_t **dimValuesPtr
   *hllVectorSizePtr = (size_t)totals[1];
   *hllDimRegIDCountPtr = static_cast<uint16_t *>(cnt);
   return dims;
+}
+
+// Arguments of finalizeSmallKernel / exportToPeersKernel for an output block of `capacity` rows; the exchange form
+// (ordered = 0) unless the caller says otherwise.
+static SmallFinalizeArgs smallFinalizeArgs(const AggState *st, int capacity, uint8_t *outBlock, uint8_t *outValues, uint32_t *resultDev) {
+  SmallFinalizeArgs A;
+  memset(&A, 0, sizeof(A));
+  A.G = st->table;
+  A.L = makeDimLayout(st->spec.NumDimsPerDimWidth, capacity);
+  A.outBlock = outBlock; A.outValues = outValues; A.resultDev = resultDev;
+  A.rowBytes = st->rowLayout.rowBytes; A.width = st->measWidth; A.outCapacity = capacity;
+  A.keyMode = st->keyMode; A.hashBits = (uint8_t)st->hashBits; A.op = st->op;
+  return A;
 }
 
 static int64_t finalize(AggState *st, const DimensionVector &out, uint8_t *outValues, cudaStream_t s, bool ordered = true) {
@@ -2210,21 +2179,16 @@ static int64_t finalize(AggState *st, const DimensionVector &out, uint8_t *outVa
   if (st->spec.ExpectedGroups <= (uint32_t)kSmallFinalizeMax && out.VectorCapacity > 0) {
     // results of up to 32768 groups: ONE launch (claim list -> hash -> sort -> merge -> emit) and ONE synchronise;
     // the group count comes back through mapped pinned memory
-    SmallFinalizeArgs A;
-    memset(&A, 0, sizeof(A));
-    A.G = st->table;
-    A.L = makeDimLayout(out.NumDimsPerDimWidth, out.VectorCapacity);
+    SmallFinalizeArgs A = smallFinalizeArgs(st, out.VectorCapacity, out.DimValues, outValues, st->resultDev);
     A.hashMask = testHash64Mask();
     A.hashA = reinterpret_cast<uint64_t *>(st->smallScratch);
     A.tmpK = A.hashA + kSmallFinalizeMax;
     A.idxA = reinterpret_cast<uint32_t *>(A.tmpK + kSmallFinalizeMax);
     A.tmpI = A.idxA + kSmallFinalizeMax;
     A.hist = A.tmpI + kSmallFinalizeMax;
-    A.outBlock = out.DimValues; A.outValues = outValues;
     A.outHash = ordered ? out.HashValues : nullptr; A.outIndex = out.IndexVector;
-    A.resultDev = st->resultDev; A.resultHost = st->resultHostDev;
-    A.rowBytes = st->rowLayout.rowBytes; A.width = width; A.outCapacity = out.VectorCapacity;
-    A.keyMode = st->keyMode; A.hashBits = (uint8_t)st->hashBits; A.op = st->op; A.plusZero = plusZero; A.ordered = ordered;
+    A.resultHost = st->resultHostDev;
+    A.plusZero = plusZero; A.ordered = ordered;
     finalizeSmallKernel<<<kFinCtas, 1024, 0, s>>>(A);
     checkLastError("finalizeSmall");
     ARES_CUDA(cudaStreamSynchronize(s));
@@ -2234,7 +2198,7 @@ static int64_t finalize(AggState *st, const DimensionVector &out, uint8_t *outVa
       return finalize(st, out, outValues, s, ordered);
     }
     if (status == SF_OK) return st->resultHost[0];
-    if (status == SF_TABLE_OVERFLOW) { const uint32_t c[2] = {st->resultHost[2], 1}; checkOverflow(st, c); }
+    if (status == SF_TABLE_OVERFLOW) checkOverflow(st, 1);
     if (status == SF_OUTPUT_TOO_SMALL) throw EngineError("output DimensionVector capacity is smaller than the number of groups");
     if (status == SF_PEER_LATE) throw EngineError("exchange over peer memory: a peer's part did not arrive within the wait bound");
     if (status == SF_PART_TRUNCATED) throw EngineError("exchange part truncated: a rank held more rows than the fixed part carries; repeat the exchange with exact sizes");
@@ -2294,6 +2258,18 @@ static int64_t finalize(AggState *st, const DimensionVector &out, uint8_t *outVa
   return g;
 }
 
+// Folds the exchange parts (AggStateMergeParts / AggStateMergePartsWhenFlagged: `flags` != nullptr) with one launch.
+static void mergeParts(AggState *st, const char *fn, const uint8_t *parts, int numParts, size_t partStride, int capRows, size_t dimOffset,
+                       size_t valuesOffset, const uint32_t *flags, uint32_t epoch, cudaStream_t s) {
+  if (st->hll) throw EngineError(std::string(fn) + ": HLL states exchange through AggStateExport");
+  if (numParts <= 0) return;
+  ensureRoom(st, (uint64_t)numParts * (uint64_t)capRows, s);
+  DimLayout L = makeDimLayout(st->spec.NumDimsPerDimWidth, capRows);
+  mergePartsKernel<<<smCount() * 2, 256, 0, s>>>(parts, numParts, partStride, dimOffset, valuesOffset, L, st->measWidth, st->op,
+                                                 st->keyMode, (uint8_t)st->hashBits, st->table, flags, epoch);
+  checkLastError(fn);
+}
+
 // HLL state -> the reference's final outputs.  AggStateFinalize on such a state already yields the
 // carried form (one row per (group, register) entry, key-ascending, value = max rho << 16 | reg);
 // this runs it into scratch buffers and then the shared register-vector stage of hll.cu.  The dim
@@ -2321,12 +2297,12 @@ static int64_t finalizeHLL(AggState *st, uint8_t **dimValuesPtr, uint8_t **hllVe
   const int dims = hllRegisterVectors(hash.as<uint64_t>(), values.as<uint32_t>(), index.as<uint32_t>(), n, hllVectorPtr,
                                       hllVectorSizePtr, hllDimRegIDCountPtr, s);
   void *out = nullptr;
-  CGoCallResHandle h = deviceMalloc(&out, (size_t)rowBytes * dims);
-  if (h.pStrErr) {
-    std::string m(h.pStrErr); free((void *)h.pStrErr);
+  try {
+    out = deviceAllocOrThrow((size_t)rowBytes * dims);
+  } catch (...) {
     deviceFree(*hllVectorPtr); deviceFree(*hllDimRegIDCountPtr);
     *hllVectorPtr = nullptr; *hllDimRegIDCountPtr = nullptr;
-    throw EngineError(m);
+    throw;
   }
   DimLayout Lin = makeDimLayout(carried.NumDimsPerDimWidth, n), Lout = makeDimLayout(carried.NumDimsPerDimWidth, dims);
   gatherDims(block.as<uint8_t>(), Lin, index.as<uint32_t>(), dims, static_cast<uint8_t *>(out), Lout, s);
@@ -2403,15 +2379,8 @@ CGoCallResHandle AggStateExportPart(void *state, uint8_t *part, int capRows, siz
     AggState *st = asState(state);
     if (st->hll) throw EngineError("AggStateExportPart: HLL states exchange through AggStateExport");
     if (capRows <= 0 || capRows > kSmallFinalizeMax) throw EngineError("AggStateExportPart: capRows must be in [1, 32768]");
-    SmallFinalizeArgs A;
-    memset(&A, 0, sizeof(A));
-    A.G = st->table;
-    A.L = makeDimLayout(st->spec.NumDimsPerDimWidth, capRows);
-    A.hashMask = ~0ull;
-    A.outBlock = part + dimOffset; A.outValues = part + valuesOffset;
-    A.resultDev = reinterpret_cast<uint32_t *>(part); A.resultHost = st->resultHostDev + 4;   // host copy unused
-    A.rowBytes = st->rowLayout.rowBytes; A.width = st->measWidth; A.outCapacity = capRows;
-    A.keyMode = st->keyMode; A.hashBits = (uint8_t)st->hashBits; A.op = st->op; A.plusZero = 0; A.ordered = 0;
+    SmallFinalizeArgs A = smallFinalizeArgs(st, capRows, part + dimOffset, part + valuesOffset, reinterpret_cast<uint32_t *>(part));
+    A.resultHost = st->resultHostDev + 4;   // host copy unused
     finalizeSmallKernel<<<kFinCtas, 1024, 0, (cudaStream_t)cudaStream>>>(A);
     checkLastError("AggStateExportPart");
     return 0;
@@ -2423,14 +2392,8 @@ CGoCallResHandle AggStateExportPart(void *state, uint8_t *part, int capRows, siz
 CGoCallResHandle AggStateMergeParts(void *state, const uint8_t *parts, int numParts, size_t partStride, int capRows,
                                     size_t dimOffset, size_t valuesOffset, void *cudaStream, int device) {
   return guarded("AggStateMergeParts", device, [&]() -> int64_t {
-    AggState *st = asState(state);
-    if (numParts <= 0) return 0;
-    ensureRoom(st, (uint64_t)numParts * (uint64_t)capRows, (cudaStream_t)cudaStream);
-    DimLayout L = makeDimLayout(st->spec.NumDimsPerDimWidth, capRows);
-    mergePartsKernel<<<smCount() * 2, 256, 0, (cudaStream_t)cudaStream>>>(parts, numParts, partStride, dimOffset, valuesOffset, L,
-                                                                         st->measWidth, st->op, st->keyMode, (uint8_t)st->hashBits,
-                                                                         st->hll ? (st->hllDense ? 2 : 1) : 0, st->table, nullptr, 0u);
-    checkLastError("AggStateMergeParts");
+    mergeParts(asState(state), "AggStateMergeParts", parts, numParts, partStride, capRows, dimOffset, valuesOffset, nullptr, 0u,
+               (cudaStream_t)cudaStream);
     return 0;
   });
 }
@@ -2451,12 +2414,7 @@ CGoCallResHandle AggStateExportPartToPeers(void *state, uint8_t *const *peerSlot
     memset(&E, 0, sizeof(E));
     for (int r = 0; r < numPeers; r++) { E.peerSlot[r] = peerSlots[r]; E.peerFlag[r] = peerFlags[r]; }
     uint8_t *part = peerSlots[myRank];
-    E.F.G = st->table;
-    E.F.L = makeDimLayout(st->spec.NumDimsPerDimWidth, capRows);
-    E.F.outBlock = part + dimOffset; E.F.outValues = part + valuesOffset;
-    E.F.resultDev = reinterpret_cast<uint32_t *>(part);
-    E.F.rowBytes = st->rowLayout.rowBytes; E.F.width = st->measWidth; E.F.outCapacity = capRows;
-    E.F.keyMode = st->keyMode; E.F.hashBits = (uint8_t)st->hashBits; E.F.op = st->op;
+    E.F = smallFinalizeArgs(st, capRows, part + dimOffset, part + valuesOffset, reinterpret_cast<uint32_t *>(part));
     E.partBytes = partBytes; E.numPeers = (uint32_t)numPeers; E.myRank = (uint32_t)myRank; E.epoch = epoch;
     exportToPeersKernel<<<kFinCtas, 1024, 0, (cudaStream_t)cudaStream>>>(E);
     checkLastError("AggStateExportPartToPeers");
@@ -2470,15 +2428,9 @@ CGoCallResHandle AggStateMergePartsWhenFlagged(void *state, const uint8_t *parts
                                                size_t dimOffset, size_t valuesOffset, const uint32_t *flags, uint32_t epoch,
                                                void *cudaStream, int device) {
   return guarded("AggStateMergePartsWhenFlagged", device, [&]() -> int64_t {
-    AggState *st = asState(state);
-    if (numParts <= 0) return 0;
     if (flags == nullptr) throw EngineError("AggStateMergePartsWhenFlagged: flags is null");
-    ensureRoom(st, (uint64_t)numParts * (uint64_t)capRows, (cudaStream_t)cudaStream);
-    DimLayout L = makeDimLayout(st->spec.NumDimsPerDimWidth, capRows);
-    mergePartsKernel<<<smCount() * 2, 256, 0, (cudaStream_t)cudaStream>>>(parts, numParts, partStride, dimOffset, valuesOffset, L,
-                                                                         st->measWidth, st->op, st->keyMode, (uint8_t)st->hashBits,
-                                                                         0, st->table, flags, epoch);
-    checkLastError("AggStateMergePartsWhenFlagged");
+    mergeParts(asState(state), "AggStateMergePartsWhenFlagged", parts, numParts, partStride, capRows, dimOffset, valuesOffset, flags,
+               epoch, (cudaStream_t)cudaStream);
     return 0;
   });
 }

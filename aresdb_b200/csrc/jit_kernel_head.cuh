@@ -85,27 +85,6 @@ __device__ __forceinline__ void ldq(const uint8_t *vals, uint32_t q, uint32_t (&
   }
 }
 
-// Gather forms (compacted survivors: four arbitrary rows of the tile): same results as ldq / ldbits for rows[0..3].
-template <int W, bool SIGNED>
-__device__ __forceinline__ void ldqg(const uint8_t *vals, const uint32_t (&rows)[4], uint32_t (&v)[4]) {
-#pragma unroll
-  for (int r = 0; r < 4; r++) {
-    if (W == 4) v[r] = reinterpret_cast<const uint32_t *>(vals)[rows[r]];
-    else if (W == 2) v[r] = SIGNED ? (uint32_t)(int32_t)reinterpret_cast<const int16_t *>(vals)[rows[r]] : reinterpret_cast<const uint16_t *>(vals)[rows[r]];
-    else v[r] = SIGNED ? (uint32_t)(int32_t)reinterpret_cast<const int8_t *>(vals)[rows[r]] : vals[rows[r]];
-  }
-}
-template <int START_BIT>
-__device__ __forceinline__ uint32_t ldbitsg(const uint8_t *bits, const uint32_t (&rows)[4]) {
-  uint32_t nib = 0;
-#pragma unroll
-  for (int r = 0; r < 4; r++) {
-    const uint32_t bit = rows[r] + START_BIT;
-    nib |= ((bits[bit >> 3] >> (bit & 7)) & 1u) << r;
-  }
-  return nib;
-}
-
 // 4 consecutive bits (rows 4q..4q+3) of a bit-packed vector whose row 0 sits at bit START_BIT
 template <int START_BIT>
 __device__ __forceinline__ uint32_t ldbits(const uint8_t *bits, uint32_t q) {

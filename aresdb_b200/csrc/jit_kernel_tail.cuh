@@ -67,11 +67,10 @@ static __device__ __noinline__ void denseColdRows(const uint8_t *stage, uint32_t
 }
 
 // Where the accumulators of the direct-indexed slots live (JIT_DENSE_ACC, chosen by the host):
-//   0  the CTA's private slice of global memory, updated with fire-and-forget RED (one L2 atomic per row);
-//   1  shared memory (native ATOMS for 4-byte aggregates, a CAS loop for 8-byte ones);
-//   2  both: row positions 0-1 of a quad go to shared memory, 2-3 to the L2 slice, so that neither the SM's
-//      shared-memory atomic path nor its global-atomic path carries the whole stream; the flush adds the two halves;
-//   3  as 2 with three row positions in shared memory and one in the L2 slice;
+//   1  shared memory (native ATOMS): 4-byte aggregates other than float min / max;
+//   2  the others: row positions 0-1 of a quad go to shared memory (a CAS loop), 2-3 to the CTA's private slice of
+//      global memory (fire-and-forget RED), so that neither the SM's shared-memory atomic path nor its global-atomic
+//      path carries the whole stream; the flush adds the two halves;
 //   4  exact integer accumulation of a bounded float sum (three 32-bit counters per slot).
 constexpr uint32_t kDenseCap = JIT_SMEM_SLOTS;   // a multiple of 16; JIT_TABLE_BYTES >= 9 * kDenseCap
 // layout of the table region (dynamic shared memory + 128) in this mode: touched[kDenseCap] | acc[kDenseCap] (8 bytes each)
@@ -239,7 +238,7 @@ __device__ __forceinline__ void jitAggregateDense(uint32_t touchedAddr, unsigned
     const uint32_t sAccAddr = touchedAddr + kDenseCap;
     // (issuing the compare-and-swap loops of the shared-memory rows interleaved instead of one after the other was
     // measured and changed nothing: 0.376 vs 0.372 ms on cfg3)
-    constexpr int kToShared = JIT_DENSE_ACC == 1 ? 4 : JIT_DENSE_ACC == 2 ? 2 : JIT_DENSE_ACC == 3 ? 3 : 0;   // row positions 0 .. kToShared-1
+    constexpr int kToShared = JIT_DENSE_ACC == 1 ? 4 : 2;   // row positions 0 .. kToShared-1
 #pragma unroll
     for (int r = 0; r < 4; r++) {
       if (r < kToShared) redSharedPred<JIT_AGG_OP>(sAccAddr + 8u * s[r], denseSharedAcc() + s[r], meas[r], go[r]);
@@ -341,7 +340,7 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
     if (JIT_DENSE_ACC == 4) {
       uint32_t *c = reinterpret_cast<uint32_t *>(tKeys) + 3u * i;
       c[0] = 0; c[1] = 0; c[2] = 0;
-    } else if (JIT_DENSE_ACC != 0) {
+    } else {
       denseSharedAcc()[i] = P.accNeutral;
     }
   }
@@ -354,10 +353,6 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
   if (threadIdx.x == 0) {
     *claims = 0;
     *misses = 0;
-    reinterpret_cast<uint32_t *>(smem + 76)[0] = 0;   // compaction cursors / stop words (JIT_COMPACT)
-    reinterpret_cast<uint32_t *>(smem + 76)[1] = 0;
-    reinterpret_cast<uint32_t *>(smem + 76)[2] = 0;
-    reinterpret_cast<uint32_t *>(smem + 76)[3] = 0;
     if (JIT_PARTITION) {   // partition histogram / fill cursors
       uint32_t *h = reinterpret_cast<uint32_t *>(smem + 128 + JIT_SMEM_SLOTS * 8);
       for (int i = 0; i < 3 * (int)kPartitionsJ + 2; i++) h[i] = 0;
@@ -405,7 +400,7 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
       // (read before the wait: the L2 round trip overlaps with it; a slightly older value only delays the stop by a tile)
       const uint32_t stopFlag = kCanDrain ? __ldcg(&P.G.counters[3]) : 0u;   // (L2, not system scope)
       mbarWait(&bars[s], parity);
-      if (!JIT_COMPACT && !draining && it >= myStart && stopFlag != 0u) {   // (compacted form: decided CTA-wide below)
+      if (!draining && it >= myStart && stopFlag != 0u) {
         draining = true;
         foldedUntil = it;
       }
@@ -429,52 +424,6 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
         if (rowEval(stage, q, t * JIT_TILE_ROWS + q * 4, P, 4u, fast, anySlow, dslot, meas, mraw))
           jitAggregateDense(touchedAddr, tAcc, P, stage, q, t * JIT_TILE_ROWS + q * 4, 4u, repOff, fast, anySlow, dslot, meas, mraw);
         (void)allowClaim; (void)bypass;
-#elif JIT_COMPACT
-        // Compacted index vector (warp ballot + prefix sum): pass 1 evaluates ONLY the filters of the thread's quad and
-        // appends the surviving rows' tile positions to a CTA-wide list — a warp reserves its span with one add on the
-        // shared cursor, lanes place their rows by an in-warp prefix sum; pass 2 hands the list out four rows per thread
-        // and evaluates dimensions / measure / aggregation on those only, so the expensive part runs on dense quads
-        // (roughly `selectivity` of the warps do it, the rest skip).  One named barrier per tile among the consumers:
-        // list and cursor are double-buffered by tile parity.  The growth stop is decided CTA-wide here (every warp
-        // must reach the barrier): thread 0's view of the flag, published before the barrier.
-        (void)meas;
-        const uint32_t par = it & 1u;
-        uint16_t *list = reinterpret_cast<uint16_t *>(smem + 128 + JIT_SMEM_SLOTS * 8) + par * 4096u;
-        uint32_t *cursor = reinterpret_cast<uint32_t *>(smem + 76) + par;       // smem + 76, + 80
-        uint32_t *stopWord = reinterpret_cast<uint32_t *>(smem + 84) + par;     // smem + 84, + 88
-        const uint32_t alive = rowAlive(stage, q, t * JIT_TILE_ROWS + q * 4, P);
-        const uint32_t lane = threadIdx.x & 31u;
-        uint32_t incl = __popc(alive);
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          const uint32_t up = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-          if ((int)lane >= o) incl += up;
-        }
-        uint32_t base = 0;
-        if (lane == 31) base = atomicAdd(cursor, incl);
-        base = __shfl_sync(0xFFFFFFFFu, base, 31) + incl - __popc(alive);
-#pragma unroll
-        for (int r = 0; r < 4; r++)
-          if ((alive >> r) & 1u) list[base++] = (uint16_t)(q * 4 + r);
-        if (threadIdx.x == 0) {
-          *stopWord = kCanDrain ? stopFlag : 0u;
-          reinterpret_cast<uint32_t *>(smem + 76)[par ^ 1u] = 0;   // the other tile's cursor: nobody touches it until after the next barrier
-        }
-        asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory");
-        if (*reinterpret_cast<volatile uint32_t *>(stopWord) != 0u) {
-          draining = true;
-          foldedUntil = it;
-        } else {
-          const uint32_t nAlive = *reinterpret_cast<volatile uint32_t *>(cursor);
-          for (uint32_t j = threadIdx.x; j * 4 < nAlive; j += kConsumerThreads) {
-            uint32_t rows4[4];
-#pragma unroll
-            for (int r = 0; r < 4; r++) rows4[r] = j * 4 + r < nAlive ? (uint32_t)list[j * 4 + r] : 0xFFFFu;
-            uint64_t key[4][JIT_KW], m2[4];
-            const uint32_t a2 = rowEvalGather(stage, rows4, t * JIT_TILE_ROWS, P, key, m2);
-            jitAggregate(T, P, a2, key, m2, allowClaim, bypass, misses);
-          }
-        }
 #elif JIT_PARTITION
         // Radix-partitioned aggregation, pass 1 (the group table is far beyond L2: a random atomic per row would miss it
         // every time).  The tile's surviving rows become (key, measure) entries, counting-sorted in shared memory by the
@@ -610,7 +559,7 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
       const uint32_t *c = reinterpret_cast<const uint32_t *>(tKeys) + 3u * i;
       const unsigned long long v = (unsigned long long)c[0] + ((unsigned long long)c[1] << 11) + ((unsigned long long)c[2] << 22);
       if (v != 0) accS = (unsigned long long)__double_as_longlong(__ull2double_rn(v) * P.fxInv);
-    } else if (JIT_DENSE_ACC != 0) {
+    } else {
       accS = denseSharedAcc()[i];
     }
     const unsigned long long accG = JIT_DENSE_ACC != 1 ? __ldcg(&tAcc[i]) : P.accNeutral;
@@ -629,7 +578,7 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
     const unsigned long long k = jitKeyOfRow(key);
     // (the host does not wait for these kernels: when the table is at its growth threshold new groups are parked)
     if (JIT_DENSE_ACC != 1) globalUpdate(P.G, (AggOp)JIT_AGG_OP, k, JIT_KW == 1 ? nullptr : key, accG, true);
-    if (JIT_DENSE_ACC != 0) globalUpdate(P.G, (AggOp)JIT_AGG_OP, k, JIT_KW == 1 ? nullptr : key, accS, true);
+    globalUpdate(P.G, (AggOp)JIT_AGG_OP, k, JIT_KW == 1 ? nullptr : key, accS, true);
   }
   return;
 #endif

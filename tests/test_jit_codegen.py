@@ -217,16 +217,10 @@ def test_join_queries_specialise():
         assert "cuckooLookup(P.join->tables[0]" in src and "foreignLoad(P.join->cols[" in src
 
 
-def test_partitioned_and_compacted_forms_compile(monkeypatch):
-    """The radix-partitioned form (tables beyond L2) and the compacted-index form of the hash-table kernel compile for the
-    plans they apply to."""
+def test_partitioned_form_compiles(monkeypatch):
+    """The radix-partitioned form of the hash-table kernel (tables beyond L2) compiles for the plans it applies to."""
     lib = A.load_engine()
     monkeypatch.setenv("ARESDB_B200_PARTITION", "1")
     for name in ("cfg2", "cfg3_sum", "cfg3_count", "min_city"):
         size, src = _dry_run(lib, T.queries()[name])
         assert size > 0 and "#define JIT_PARTITION 1" in src, name
-    monkeypatch.delenv("ARESDB_B200_PARTITION")
-    monkeypatch.setenv("ARESDB_B200_COMPACT", "1")
-    for name in ("cfg2", "cfg3_sum", "cfg3_count"):
-        size, src = _dry_run(lib, T.queries()[name])
-        assert size > 0 and "#define JIT_COMPACT 1" in src and "rowEvalGather" in src, name

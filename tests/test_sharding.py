@@ -137,6 +137,35 @@ def test_export_part_merge_parts_on_device():
 
 
 @pytest.mark.gpu
+def test_exchange_parts_refuse_hll_states():
+    """HLL states exchange through AggStateExport (carried rows): the fixed-size part entry points refuse them on the
+    sending and on both receiving sides, in entry and in dense-register mode."""
+    import torch
+    import harness as H
+    import test_hll_pipeline as HP
+    from aresdb_b200 import cabi as A
+    from aresdb_b200.executor import FusedBatchExecutor, dim_offsets
+    eng = H.get_backend("b200")
+    st = eng.space.stream
+    q = HP.hll_queries()["two_dims"]
+    cap = 64
+    _, _, _, dim_bytes = dim_offsets(q.num_dims_per_width, cap)
+    dim_bytes = (dim_bytes + 15) // 16 * 16
+    part = (64 + dim_bytes + q.measure_bytes * cap + 63) // 64 * 64
+    buf = torch.zeros(256 + 2 * part, dtype=torch.uint8, device=eng.space.dev)   # flags | two parts
+    parts = buf.data_ptr() + 256
+    for mode in (HP.ENTRY_MODE, HP.DENSE_MODE):
+        ex = FusedBatchExecutor(eng.lib, eng.space, q, mode)
+        with pytest.raises(A.AresError, match="AggStateExportPart: HLL states exchange through AggStateExport"):
+            eng.lib.AggStateExportPart(ex.state, parts, cap, 64, 64 + dim_bytes, st, 0)
+        with pytest.raises(A.AresError, match="AggStateMergeParts: HLL states exchange through AggStateExport"):
+            eng.lib.AggStateMergeParts(ex.state, parts, 2, part, cap, 64, 64 + dim_bytes, st, 0)
+        with pytest.raises(A.AresError, match="AggStateMergePartsWhenFlagged: HLL states exchange through AggStateExport"):
+            eng.lib.AggStateMergePartsWhenFlagged(ex.state, parts, 2, part, cap, 64, 64 + dim_bytes, buf.data_ptr(), 1, st, 0)
+        ex.close()
+
+
+@pytest.mark.gpu
 def test_exchange_over_peer_memory_kernels_on_one_device():
     """AggStateExportPartToPeers / AggStateMergePartsWhenFlagged with both "ranks" on one GPU: two states export into each
     other's receive buffers (part in the sender's slot of BOTH buffers, flag raised to the epoch on both), each receive
