@@ -1607,9 +1607,8 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups, bool allowDense 
     }
     if (!tileRows) {
       for (uint32_t sl : {slots, slots / 2, slots / 4}) {
-        if (P.partition && sl != 8192) break;      // the tile buffer of the partitioned form IS the 64 KB table region
         for (uint32_t tr : {3968u, 1920u, 896u}) {  // 128 rows x (31 | 15 | 7) consumer warps
-          size_t avail = (size_t)kSmemBudget - 128 - (size_t)sl * 8 - (P.partition ? kPartitionExtraBytes : 0u);
+          size_t avail = (size_t)kSmemBudget - 128 - (size_t)sl * 8;
           uint32_t n = (uint32_t)(avail / stageBytesFor(tr));
           if (n >= 2) { tileRows = tr; stages = n > (uint32_t)kMaxStages ? kMaxStages : n; break; }
         }
@@ -1658,9 +1657,7 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups, bool allowDense 
   P.stageBytes = (uint32_t)stageBytes;
   P.smemSlots = slots;
   P.tableBytes = P.denseNd != 0 ? (slots * (P.hll ? 4 : P.denseFx ? 12 : 9) + 127) / 128 * 128 : slots * 8;
-  if (P.denseNd != 0 || !P.staged) P.partition = 0;
-  if (P.partition && (slots != 8192 || P.tileRows > 4096)) P.partition = 0;
-  return 128 + (size_t)P.tableBytes + (P.partition ? kPartitionExtraBytes : 0u) + stageBytes * P.numStages;
+  return 128 + (size_t)P.tableBytes + stageBytes * P.numStages;
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1685,26 +1682,6 @@ __global__ void __launch_bounds__(256) mergeSpillKernel(DevTable G, uint32_t n, 
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
     const SpillEntry e = G.spill[i];
     globalUpdate(G, op, e.key, G.rows ? e.row : nullptr, e.val);
-  }
-}
-
-// Radix-partitioned aggregation, pass 2: the entries the fused kernel appended tile by tile (each tile's span sorted by
-// partition, its directory line giving the 64 segment offsets) are folded PARTITION-MAJOR: warp w takes pair
-// (partition, tile) number w, w + W, ... in that order, so that at any moment the whole grid updates the same
-// partition = one contiguous 1/64 of the table's slots, which stays in L2 while it is being worked on.
-__global__ void __launch_bounds__(256)
-partitionAggregateKernel(const uint4 *__restrict__ entries, const uint32_t *__restrict__ dir, uint32_t numTiles, AggOp op, DevTable G) {
-  const uint32_t lane = threadIdx.x & 31u;
-  const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x >> 5), pairs = (uint64_t)kPartitions * numTiles;
-  for (uint64_t idx = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); idx < pairs; idx += warps) {
-    const uint32_t p = (uint32_t)(idx / numTiles), tile = (uint32_t)(idx % numTiles);
-    const uint32_t *line = dir + (size_t)tile * kPartDirWords;
-    const uint32_t begin = line[kPartitions + 1] + line[p], end = line[kPartitions + 1] + line[p + 1];
-    for (uint32_t i = begin + lane; i < end; i += 32) {
-      const uint4 e = entries[i];
-      globalUpdate(G, op, (unsigned long long)e.x | ((unsigned long long)e.y << 32), nullptr,
-                   (uint64_t)e.z | ((uint64_t)e.w << 32), /*spillWhenStopped=*/true);
-    }
   }
 }
 
@@ -1875,27 +1852,7 @@ static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
     ARES_CUDA(cudaStreamSynchronize(s));   // J is reused by the next call of this thread
     P.join = joinMem->as<DevJoin>();
   }
-  // radix-partitioned aggregation when the table is far beyond L2 (or ARESDB_B200_PARTITION=1): packed keys, plain sums /
-  // min / max, specialised kernel only
-  {
-    const char *e = getenv("ARESDB_B200_PARTITION");
-    const bool want = e ? e[0] == '1' : st->capacity >= kPartitionMinSlots;
-    P.partition = want && jitAvailable() && st->keyMode == KEY_PACKED && !st->hll && P.numForeignCols == 0 && st->capacity >= 4096;
-    int lg = 0;
-    while (((size_t)1 << lg) < st->capacity) lg++;
-    P.partShift = (uint8_t)(lg > 6 ? lg - 6 : 0);
-  }
   size_t smemBytes = layoutStages(P, st->spec.ExpectedGroups);
-  std::unique_ptr<Scratch> partMem;
-  if (P.partition) {
-    const size_t dirBytes = ((size_t)P.numFullTiles * kPartDirWords * 4 + 255) / 256 * 256;
-    partMem.reset(new Scratch(256 + dirBytes + (size_t)P.numRows * sizeof(uint4), s));
-    uint8_t *pm = partMem->as<uint8_t>();
-    P.partCursor = reinterpret_cast<uint32_t *>(pm);
-    P.partDir = reinterpret_cast<uint32_t *>(pm + 256);
-    P.partBuf = reinterpret_cast<uint4 *>(pm + 256 + dirBytes);
-    ARES_CUDA(cudaMemsetAsync(pm, 0, 256, s));
-  }
   // per-tile run hints of the first-class RLE columns (the tile size is known now)
   for (int c = 0; c < P.ncols; c++) {
     DevColumn &col = P.cols[c];
@@ -1911,7 +1868,7 @@ static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
   // room in the group table (see "growth of the group table"): the direct path and the direct-indexed kernels are not
   // waited for, so what they may insert is reserved up front (flush of the CTA slots / fold of the global slot array;
   // out-of-range rows park); hash-table tile kernels are checked after the launch and resumed when they stopped.
-  const bool resumable = P.staged && P.denseNd == 0 && !st->hllDense && !P.partition;
+  const bool resumable = P.staged && P.denseNd == 0 && !st->hllDense;
   if (!resumable && !st->hllDense) ensureRoom(st, P.staged ? (uint64_t)P.denseTotal : (uint64_t)P.numRows, s);
   P.ctaAcc = st->ctaAcc;   // (after a possible growth: the slices live in the table's allocation)
   static bool attrSet[64] = {false};
@@ -1941,15 +1898,6 @@ static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
     bool checkAfter = false;   // a hash-table tile kernel ran: wait for it and resume it if the table stopped it
     if (P.staged && jitLaunchStaged(P, st->table, smemBytes, grid, s)) {
       checkAfter = P.denseNd == 0 && !st->hllDense;
-      if (P.partition) {   // pass 2: fold the entries partition by partition; the table is checked (and grown) after every batch
-        partitionAggregateKernel<<<smCount() * 8, 256, 0, s>>>(P.partBuf, P.partDir, P.numFullTiles, (AggOp)P.aggOp, st->table);
-        checkLastError("partitionAggregate");
-        const TableCounters c = readCounters(st, s);
-        st->everChecked = true;
-        checkOverflow(st, c.overflow);
-        if (c.stop || c.spilled) settleTable(st, s);
-        return;
-      }
       if (P.denseGlobal) {
         DenseFold F;
         memset(&F, 0, sizeof(F));
@@ -2473,10 +2421,6 @@ CGoCallResHandle AresJitDryRun(AggSpec spec, const BatchPlan *plan, char **sourc
     static thread_local DevPlan P;
     compilePlan(&st, *plan, P);
     P.tailBegin = 0;
-    if (const char *e = getenv("ARESDB_B200_PARTITION")) {   // the partitioned form of the kernel (normally chosen by table size)
-      P.partition = e[0] == '1' && st.keyMode == KEY_PACKED && !st.hll && P.numForeignCols == 0;
-      P.partShift = 15;
-    }
     layoutStages(P, spec.ExpectedGroups);
     std::string src;
     size_t n = P.staged ? jitCompileOnly(P, &src) : 0;

@@ -53,13 +53,9 @@ struct JitParams {
   float fxScale;                          //                     2^S (a float sum's rows are added as integers x * 2^S)
   uint32_t fxPad;
   const DevJoin *join;                    // joined dimension tables (join.cuh), null without joins
-  uint32_t resume;
+  uint32_t resume;                        // 1: second launch of the same batch after the table grew (progress[] says where)
   uint32_t startCount;                    // row number of index position 0 when the batch has no base counts
-  uint32_t partShift;                     // JIT_PARTITION: partition = home slot >> partShift
-  uint4 *partBuf;                         //   entries (key, measure) of this batch, tile by tile, sorted by partition inside a tile
-  uint32_t *partDir;                      //   per tile: segment offsets + span base
-  uint32_t *partCursor;                   //   entries appended so far
-  RleColumn rle[kJitMaxRle];              // run-length encoded columns decoded in place (see ldrle)                        // 1: second launch of the same batch after the table grew (progress[] says where)
+  RleColumn rle[kJitMaxRle];              // run-length encoded columns decoded in place (see ldrle)
 };
 
 

@@ -6,8 +6,6 @@
 // rowEval() precede this text.
 namespace aresb {
 
-constexpr uint32_t kPartitionsJ = 64;   // = kPartitions (plan_device.cuh)
-
 __device__ __forceinline__ void jitIssueTile(const JitParams &P, uint32_t tile, uint8_t *stage, uint64_t *bar) {
   mbarExpectTx(bar, JIT_STAGE_TX_BYTES);
 #pragma unroll
@@ -353,10 +351,6 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
   if (threadIdx.x == 0) {
     *claims = 0;
     *misses = 0;
-    if (JIT_PARTITION) {   // partition histogram / fill cursors
-      uint32_t *h = reinterpret_cast<uint32_t *>(smem + 128 + JIT_SMEM_SLOTS * 8);
-      for (int i = 0; i < 3 * (int)kPartitionsJ + 2; i++) h[i] = 0;
-    }
     for (int s = 0; s < JIT_STAGES; s++) {
       mbarInit(&bars[s], 1);
       mbarInit(&empty[s], JIT_THREADS / 32 - 1);
@@ -378,7 +372,7 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
   // lost and nothing is counted twice; the unit is one warp's 128 rows of one tile.
   // (Direct-indexed kernels never drain — the host does not wait for them: their out-of-range rows and their flush park
   // new groups in DevTable::spill while the table is at its threshold.)
-  constexpr bool kCanDrain = JIT_DENSE == 0 && JIT_PARTITION == 0;   // (the partitioned form inserts nothing in this kernel)
+  constexpr bool kCanDrain = JIT_DENSE == 0;
   const uint32_t progIdx = blockIdx.x * kProgressWarps + (threadIdx.x >> 5);
   uint32_t myStart = 0;
   if (kCanDrain && P.resume) myStart = P.G.progress[progIdx];
@@ -423,61 +417,6 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
         uint32_t mraw[4];
         if (rowEval(stage, q, t * JIT_TILE_ROWS + q * 4, P, 4u, fast, anySlow, dslot, meas, mraw))
           jitAggregateDense(touchedAddr, tAcc, P, stage, q, t * JIT_TILE_ROWS + q * 4, 4u, repOff, fast, anySlow, dslot, meas, mraw);
-        (void)allowClaim; (void)bypass;
-#elif JIT_PARTITION
-        // Radix-partitioned aggregation, pass 1 (the group table is far beyond L2: a random atomic per row would miss it
-        // every time).  The tile's surviving rows become (key, measure) entries, counting-sorted in shared memory by the
-        // PARTITION of the table their home slot lies in (64 partitions = 64 contiguous slot ranges), and are appended
-        // to the batch's entry buffer in HBM as one contiguous, partition-ordered span (coalesced 16-byte writes) with a
-        // directory line saying where each partition's segment of this tile starts.  Pass 2 (partitionAggregateKernel)
-        // then folds partition after partition, so that the slot range being updated stays L2-resident.
-        static_assert(JIT_KW == 1 && JIT_HLL == 0, "partitioned form: packed keys");
-        uint4 *buf = reinterpret_cast<uint4 *>(tKeys);                                   // 3968 entries x 16 B <= 64 KB
-        uint32_t *hist = reinterpret_cast<uint32_t *>(smem + 128 + JIT_SMEM_SLOTS * 8);  // [64]
-        uint32_t *off = hist + kPartitionsJ;                                              // [65]
-        uint32_t *fill = off + kPartitionsJ + 1;                                          // [64]
-        uint32_t *span = fill + kPartitionsJ;                                             // [1]
-        uint64_t key[4][JIT_KW];
-        const uint32_t alive = rowEval(stage, q, t * JIT_TILE_ROWS + q * 4, P, key, meas);
-        uint32_t part[4];
-#pragma unroll
-        for (int r = 0; r < 4; r++) {
-          part[r] = globalHome(P.G, key[r][0]) >> P.partShift;
-          if ((alive >> r) & 1u) atomicAdd(&hist[part[r]], 1u);
-        }
-        asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory");
-        if (threadIdx.x < 32) {   // one warp: exclusive scan of the 64 counts, the tile's span in the entry buffer, its directory line
-          const uint32_t c0 = hist[2 * threadIdx.x], c1 = hist[2 * threadIdx.x + 1];
-          uint32_t incl = c0 + c1;
-#pragma unroll
-          for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t up = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-            if ((int)threadIdx.x >= o) incl += up;
-          }
-          const uint32_t ex = incl - c0 - c1, total = __shfl_sync(0xFFFFFFFFu, incl, 31);
-          uint32_t base = 0;
-          if (threadIdx.x == 0) base = atomicAdd(P.partCursor, total);
-          base = __shfl_sync(0xFFFFFFFFu, base, 0);
-          off[2 * threadIdx.x] = ex; off[2 * threadIdx.x + 1] = ex + c0;
-          hist[2 * threadIdx.x] = 0; hist[2 * threadIdx.x + 1] = 0;
-          fill[2 * threadIdx.x] = 0; fill[2 * threadIdx.x + 1] = 0;
-          uint32_t *line = P.partDir + (size_t)t * (kPartitionsJ + 2);
-          line[2 * threadIdx.x] = ex; line[2 * threadIdx.x + 1] = ex + c0;
-          if (threadIdx.x == 0) { off[kPartitionsJ] = total; *span = base; line[kPartitionsJ] = total; line[kPartitionsJ + 1] = base; }
-        }
-        asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory");
-#pragma unroll
-        for (int r = 0; r < 4; r++) {
-          if (!((alive >> r) & 1u)) continue;
-          const uint32_t pos = off[part[r]] + atomicAdd(&fill[part[r]], 1u);
-          buf[pos] = make_uint4((uint32_t)key[r][0], (uint32_t)(key[r][0] >> 32), (uint32_t)meas[r], (uint32_t)(meas[r] >> 32));
-        }
-        asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory");
-        {
-          const uint32_t total = off[kPartitionsJ], base = *span;
-          for (uint32_t i = threadIdx.x; i < total; i += kConsumerThreads) P.partBuf[base + i] = buf[i];
-        }
-        asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory");
         (void)allowClaim; (void)bypass;
 #else
         uint64_t key[4][JIT_KW];
@@ -534,12 +473,7 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
         uint64_t key[4][JIT_KW];
         uint32_t alive = rowEval(stages, q, done + q * 4, P, key, meas);
         alive &= (1u << nvalid) - 1u;
-#if JIT_PARTITION
-        for (int r = 0; r < 4; r++)   // (the shared table region is the tile buffer in this form: straight to the global table)
-          if ((alive >> r) & 1u) globalUpdate(P.G, (AggOp)JIT_AGG_OP, jitKeyOf(key, meas, r), nullptr, meas[r], /*spillWhenStopped=*/true);
-#else
         jitAggregate(T, P, alive, key, meas, true, false, misses);
-#endif
 #endif
       }
       done += rows;
@@ -583,7 +517,7 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
   return;
 #endif
   // (the CTA's table is folded whatever the state of the global one: groups it cannot take right now are parked)
-  for (uint32_t i = threadIdx.x; i < (JIT_PARTITION ? 0u : (uint32_t)JIT_SMEM_SLOTS); i += JIT_THREADS) {
+  for (uint32_t i = threadIdx.x; i < JIT_SMEM_SLOTS; i += JIT_THREADS) {
     unsigned long long k = tKeys[i];
     if (k != kEmptyKey) globalUpdate(P.G, (AggOp)JIT_AGG_OP, k, nullptr, __ldcg(&tAcc[i]), /*spillWhenStopped=*/true);
   }

@@ -101,12 +101,6 @@ struct DevPlan {
   uint8_t foreignClass[kMaxForeignCols];    // ValClass a read of foreign column k yields
   uint8_t pad2[1];
   const DevJoin *join;     // device copy of the tables' indexes and the foreign columns' batches
-  uint8_t partition;       // radix-partitioned aggregation (tables beyond L2): the kernel emits (key, measure) entries sorted by
-                           // table partition, a second kernel folds them partition by partition
-  uint8_t partShift;       // partition of a key = its home slot >> partShift (64 partitions)
-  uint4 *partBuf;          // [numRows] entries of this batch
-  uint32_t *partDir;       // [numFullTiles][kPartDirWords]: per tile, offsets of the 64 partition segments + span base
-  uint32_t *partCursor;    // entries appended so far
   uint32_t resume;         // 1: relaunch of the same batch after the group table grew (DevTable::progress holds the resume points)
 };
 
@@ -118,10 +112,6 @@ constexpr uint32_t kGlobalDenseMaxSlots = 1u << 21;   // 16 MB of accumulators p
 // when NVRTC is unavailable or disabled (ARESDB_B200_JIT=0) so that the caller falls back to the
 // interpreter kernel; throws EngineError when code generation / compilation fails.
 bool jitAvailable();
-constexpr uint32_t kPartitions = 64;
-constexpr uint32_t kPartDirWords = kPartitions + 2;   // off[0..64] (off[64] = entries of the tile), span base
-constexpr uint32_t kPartitionExtraBytes = 2048;   // histogram / offsets / fill cursors behind the 64 KB tile buffer
-constexpr size_t kPartitionMinSlots = (size_t)1 << 23;   // tables from 8M slots (>= 128 MB of keys + accumulators: beyond L2)
 void jitAnalyzeDense(DevPlan &P, bool bypass);
 size_t jitCompileOnly(const DevPlan &P, std::string *sourceOut);
 bool jitLaunchStaged(const DevPlan &P, const DevTable &G, size_t smemBytes, int grid, cudaStream_t s);

@@ -215,12 +215,3 @@ def test_join_queries_specialise():
         size, src = _dry_run(lib, q)
         assert size > 0, name
         assert "cuckooLookup(P.join->tables[0]" in src and "foreignLoad(P.join->cols[" in src
-
-
-def test_partitioned_form_compiles(monkeypatch):
-    """The radix-partitioned form of the hash-table kernel (tables beyond L2) compiles for the plans it applies to."""
-    lib = A.load_engine()
-    monkeypatch.setenv("ARESDB_B200_PARTITION", "1")
-    for name in ("cfg2", "cfg3_sum", "cfg3_count", "min_city"):
-        size, src = _dry_run(lib, T.queries()[name])
-        assert size > 0 and "#define JIT_PARTITION 1" in src, name

@@ -61,17 +61,6 @@ for case in {cases!r}:
       got = T.run_fused(eng, q, small, zone_maps=zms)
       assert T.dense_launches(eng) - before == 2 and exp.groups > 4096
       T.assert_same_result(got, exp, ctx=case)
-  elif case == "partition":   # radix-partitioned aggregation forced on (ARESDB_B200_PARTITION=1): entries sorted by table partition per
-      # tile, folded partition by partition — same results as the direct form, for sums / counts / min, few and many groups
-      big = [synth.generate_batch(d, 700000, num_cities=120, null_rate=0.02) for d in range(2)]
-      qs = dict(unique=AggQuery([E.ne(CITY, E.Lit(0))], [TS, CITY], Measure("sum", FARE)),
-                cfg3=AggQuery([E.eq(STATUS, E.Lit(1)), E.gt(FARE, E.Lit(5.0))], [E.floor(TS, E.Lit(3600)), CITY], Measure("sum", FARE)),
-                count=AggQuery([], [CITY, STATUS], Measure("count")),
-                minc=AggQuery([E.eq(STATUS, E.Lit(2))], [E.floor(TS, E.Lit(60))], Measure("min", CITY)))
-      for name, q in qs.items():
-          exp = T.run_legacy(orc, q, big)
-          got = T.run_fused(eng, q, big)
-          assert (got.packed_rows() == exp.packed_rows()).all() and got.measures.tobytes() == exp.measures.tobytes(), name
   elif case == "merge":     # AggStateMerge of more rows than the table holds
       from aresdb_b200.executor import FusedBatchExecutor
       q = AggQuery([], [TS, CITY], Measure("count"))
@@ -93,26 +82,22 @@ print("ok")
 """
 
 
-# one child process per ENVIRONMENT (table size, JIT on / off, partitioned form), several cases in it: a child pays for
-# the interpreter start-up, the library load and the NVRTC compiles once
+# one child process per ENVIRONMENT (table size, JIT on / off), several cases in it: a child pays for the interpreter
+# start-up, the library load and the NVRTC compiles once
 GROUPS = [
-    ("slots17-jit", ["hash", "hash32"], 1 << 17, "1", False),
-    ("slots17-interpreter", ["hash", "hash32"], 1 << 17, "0", False),
-    ("default-jit", ["hash_big"], 0, "1", False),
-    ("default-interpreter", ["hash_big"], 0, "0", False),
-    ("slots12-jit", ["spill", "merge"], 1 << 12, "1", False),
-    ("slots12-interpreter", ["merge"], 1 << 12, "0", False),
-    ("partition-default", ["partition"], 0, "1", True),
-    ("partition-slots18", ["partition"], 1 << 18, "1", True),
+    ("slots17-jit", ["hash", "hash32"], 1 << 17, "1"),
+    ("slots17-interpreter", ["hash", "hash32"], 1 << 17, "0"),
+    ("default-jit", ["hash_big"], 0, "1"),
+    ("default-interpreter", ["hash_big"], 0, "0"),
+    ("slots12-jit", ["spill", "merge"], 1 << 12, "1"),
+    ("slots12-interpreter", ["merge"], 1 << 12, "0"),
 ]
 
 
-@pytest.mark.parametrize("name,cases,slots,jit,partition", GROUPS, ids=[g[0] for g in GROUPS])
-def test_table_grows(name, cases, slots, jit, partition):
+@pytest.mark.parametrize("name,cases,slots,jit", GROUPS, ids=[g[0] for g in GROUPS])
+def test_table_grows(name, cases, slots, jit):
     code = CHILD.format(tests=str(ROOT / "tests"), root=str(ROOT), cases=cases)
     env = dict(os.environ, ARESDB_B200_JIT=jit)
-    if partition:
-        env["ARESDB_B200_PARTITION"] = "1"
     if slots:
         env["ARESDB_B200_TABLE_SLOTS"] = str(slots)
     r = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=900)
