@@ -1,17 +1,19 @@
 // batch_plan.cu — the fused whole-batch engine behind include/aresdb_b200/batch_plan.h.
 //
-// ExecuteBatchPlan = ONE persistent kernel per batch (fusedBatchKernel):
+// ExecuteBatchPlan = ONE persistent kernel per batch, specialised for the plan's shape (jit.cu,
+// jit_kernel_head.cuh / jit_kernel_tail.cuh):
 //   * column slices are staged tile by tile into shared memory by the TMA engine
 //     (cp.async.bulk global->shared, completion on an mbarrier, kStages-deep ring), so HBM is
 //     read exactly once, fully coalesced, with no LSU issue slots or registers spent on it;
-//   * every thread owns quads of 4 consecutive rows (128-bit LDS for 4-byte columns, 64-bit for
-//     2-byte, 32-bit for 1-byte, nibbles of the null bitmaps) and interprets the plan's
-//     instruction list in registers: filters clear bits of an alive mask, dimension roots pack
-//     the row key, the measure root yields the value (NULL -> identity, x RLE count);
-//   * surviving rows are aggregated into a CTA-private open-addressing table in SHARED memory
-//     (native shared atomics: tools/microbench/agg_microbench.cu measures them),
-//     which is flushed into the L2-resident global group table when the CTA retires; rows that
-//     do not fit the shared table (high cardinality) go to the global table directly.
+//     the rows after the last full tile are copied by the kernel itself;
+//   * every thread owns quads of 4 consecutive rows and evaluates the plan's instructions in
+//     registers: filters clear bits of an alive mask, dimension roots pack the row key, the
+//     measure root yields the value (NULL -> identity, x RLE count);
+//   * surviving rows are aggregated into a CTA-private table (or direct-indexed slots when the
+//     zone map bounds every dimension), which is flushed into the L2-resident global group table
+//     when the CTA retires; rows that do not fit it go to the global table directly.
+// Here: the plan's device form (compilePlan), its inputs made stageable (executePlan: run-length
+// columns, unaligned parts), the stage layout (layoutStages) and the launch / resume protocol.
 // The global table lives in an AggState across batches.  AggStateFinalize compacts it, hashes
 // each group's packed dimension row with the reference's murmur3, sorts the g groups by hash,
 // merges equal hashes and writes the reference's output layout — the observable result of the
@@ -44,496 +46,13 @@ int reduceByHash(const uint64_t *hash, const uint32_t *index, const uint8_t *mea
                  uint32_t *outIndex, uint8_t *outValues, cudaStream_t s, uint64_t *outHash = nullptr);
 
 
-// ---------------------------------------------------------------------------------------
-// 4-row vector evaluation
-// ---------------------------------------------------------------------------------------
-constexpr int R = 4;  // rows per quad
 // status word of the single-launch finalize / of an exchange part
 enum SmallFinalizeStatus : uint32_t { SF_OK = 0, SF_TOO_MANY = 1, SF_TABLE_OVERFLOW = 2, SF_OUTPUT_TOO_SMALL = 3, SF_PART_TRUNCATED = 4, SF_UNSETTLED = 5, SF_PEER_LATE = 6 };
-
-__device__ __forceinline__ void cvtVec(uint32_t (&v)[R], ValClass from, ValClass to) {
-  if (from == to) return;
-  const bool fi = from == VC_I32 || from == VC_U32 || from == VC_BOOL;
-  const bool ti = to == VC_I32 || to == VC_U32;
-  if (fi && ti) return;  // bit-identical (bool is stored as 0/1)
-#pragma unroll
-  for (int r = 0; r < R; r++) v[r] = (uint32_t)cvt(v[r], from, to);
-}
-
-// Binary functor on R rows; NULL results carry value 0 like the reference's (0, false).
-__device__ __forceinline__ void binVec(int fn, ValClass tc, const uint32_t (&a)[R], uint32_t av, const uint32_t (&b)[R],
-                                       uint32_t bv, uint32_t (&out)[R], uint32_t &ov) {
-  const uint32_t both = av & bv;
-  ov = 0;
-#define ARES_ROWS(expr_f, expr_i, expr_u)                                                                 \
-  {                                                                                                       \
-    ov = both;                                                                                            \
-    if (tc == VC_F32) {                                                                                   \
-      _Pragma("unroll") for (int r = 0; r < R; r++) {                                                     \
-        float x = __uint_as_float(a[r]), y = __uint_as_float(b[r]); (void)x; (void)y;                     \
-        out[r] = (both >> r) & 1 ? (uint32_t)(expr_f) : 0u;                                               \
-      }                                                                                                   \
-    } else if (tc == VC_I32) {                                                                            \
-      _Pragma("unroll") for (int r = 0; r < R; r++) {                                                     \
-        int32_t x = (int32_t)a[r], y = (int32_t)b[r]; (void)x; (void)y;                                   \
-        out[r] = (both >> r) & 1 ? (uint32_t)(expr_i) : 0u;                                               \
-      }                                                                                                   \
-    } else {                                                                                              \
-      _Pragma("unroll") for (int r = 0; r < R; r++) {                                                     \
-        uint32_t x = a[r], y = b[r]; (void)x; (void)y;                                                    \
-        out[r] = (both >> r) & 1 ? (uint32_t)(expr_u) : 0u;                                               \
-      }                                                                                                   \
-    }                                                                                                     \
-  }
-  switch (fn) {
-    case Equal: ARES_ROWS(x == y, x == y, x == y) return;
-    case NotEqual: ARES_ROWS(x != y, x != y, x != y) return;
-    case LessThan: ARES_ROWS(x < y, x < y, x < y) return;
-    case LessThanOrEqual: ARES_ROWS(x <= y, x <= y, x <= y) return;
-    case GreaterThan: ARES_ROWS(x > y, x > y, x > y) return;
-    case GreaterThanOrEqual: ARES_ROWS(x >= y, x >= y, x >= y) return;
-    case Plus: ARES_ROWS(__float_as_uint(__fadd_rn(x, y)), (uint32_t)x + (uint32_t)y, x + y) return;
-    case Minus: ARES_ROWS(__float_as_uint(__fsub_rn(x, y)), (uint32_t)x - (uint32_t)y, x - y) return;
-    case Multiply: ARES_ROWS(__float_as_uint(__fmul_rn(x, y)), (uint32_t)x * (uint32_t)y, x * y) return;
-    default: break;
-  }
-#undef ARES_ROWS
-  // everything else (And/Or/Divide/Mod/bitwise/Floor): scalar functor per row
-#pragma unroll
-  for (int r = 0; r < R; r++) {
-    Cell ca, cb;
-    ca.v = a[r]; ca.valid = (av >> r) & 1;
-    cb.v = b[r]; cb.valid = (bv >> r) & 1;
-    ValClass rc;
-    Cell cr = evalBinary(fn, ca, cb, tc, &rc);
-    out[r] = (uint32_t)cr.v;
-    ov = (ov & ~(1u << r)) | ((cr.valid ? 1u : 0u) << r);
-  }
-}
-
-__device__ __forceinline__ void unVec(int fn, ValClass ic, const uint32_t (&a)[R], uint32_t av, uint32_t (&out)[R],
-                                      uint32_t &ov) {
-  if (fn == Noop) {
-#pragma unroll
-    for (int r = 0; r < R; r++) out[r] = a[r];
-    ov = av;
-    return;
-  }
-  ov = 0;
-#pragma unroll
-  for (int r = 0; r < R; r++) {
-    Cell ca;
-    ca.v = a[r]; ca.valid = (av >> r) & 1;
-    ValClass rc;
-    Cell cr = evalUnary(fn, ca, ic, &rc);
-    out[r] = (uint32_t)cr.v;
-    ov = (ov & ~(1u << r)) | ((cr.valid ? 1u : 0u) << r);
-  }
-}
-
-// ---------------------------------------------------------------------------------------
-// operand fetch
-// ---------------------------------------------------------------------------------------
-// Staged: `stage` is the shared-memory copy of the tile; q is the quad index inside the tile.
-__device__ __forceinline__ void fetchStaged(const DevColumn &c, const uint8_t *stage, uint32_t q, uint32_t (&v)[R],
-                                            uint32_t &valid) {
-  const uint8_t *vals = stage + c.smemValues;
-  switch (c.width) {
-    case 4: {
-      uint4 x = *reinterpret_cast<const uint4 *>(vals + 16 * q);
-      v[0] = x.x; v[1] = x.y; v[2] = x.z; v[3] = x.w;
-      break;
-    }
-    case 2: {
-      uint2 x = *reinterpret_cast<const uint2 *>(vals + 8 * q);
-      if (c.in.dtype == Int16) {
-        v[0] = (uint32_t)(int32_t)(int16_t)(x.x & 0xffff); v[1] = (uint32_t)(int32_t)(int16_t)(x.x >> 16);
-        v[2] = (uint32_t)(int32_t)(int16_t)(x.y & 0xffff); v[3] = (uint32_t)(int32_t)(int16_t)(x.y >> 16);
-      } else {
-        v[0] = x.x & 0xffff; v[1] = x.x >> 16; v[2] = x.y & 0xffff; v[3] = x.y >> 16;
-      }
-      break;
-    }
-    case 1: {
-      uint32_t x = *reinterpret_cast<const uint32_t *>(vals + 4 * q);
-      if (c.in.dtype == Int8) {
-#pragma unroll
-        for (int r = 0; r < R; r++) v[r] = (uint32_t)(int32_t)(int8_t)((x >> (8 * r)) & 0xff);
-      } else {
-#pragma unroll
-        for (int r = 0; r < R; r++) v[r] = (x >> (8 * r)) & 0xff;
-      }
-      break;
-    }
-    default: {  // bit-packed bool
-      uint32_t bit = 4 * q + c.in.startBit;
-      uint32_t w = vals[bit >> 3] | ((uint32_t)vals[(bit >> 3) + 1] << 8);
-      w >>= (bit & 7);
-#pragma unroll
-      for (int r = 0; r < R; r++) v[r] = (w >> r) & 1;
-      break;
-    }
-  }
-  if (c.hasNulls) {
-    const uint8_t *nb = stage + c.smemNulls;
-    uint32_t bit = 4 * q + c.in.startBit;
-    uint32_t w = nb[bit >> 3] | ((uint32_t)nb[(bit >> 3) + 1] << 8);
-    valid = (w >> (bit & 7)) & 0xF;
-  } else {
-    valid = 0xF;
-  }
-}
-
-// Direct: straight from global memory, any column mode, row by row (tail tiles, unaligned or
-// RLE columns).
-__device__ __forceinline__ void fetchDirect(const DevPlan &P, const DevColumn &c, uint32_t row0, uint32_t nrows,
-                                            uint32_t (&v)[R], uint32_t &valid) {
-  valid = 0;
-#pragma unroll
-  for (int r = 0; r < R; r++) {
-    v[r] = 0;
-    if ((uint32_t)r < nrows) {
-      Cell x = loadInput(c.in, row0 + r, nullptr, P.baseCounts, P.startCount, nullptr);
-      v[r] = (uint32_t)x.v;
-      valid |= (x.valid ? 1u : 0u) << r;
-    }
-  }
-}
-
-struct QuadState {
-  uint32_t st[ARES_PLAN_STACK_DEPTH][R];
-  uint32_t stv[ARES_PLAN_STACK_DEPTH];
-};
-
-template <bool STAGED>
-__device__ __forceinline__ void getOperand(const DevPlan &P, const DevInst &I, bool second, const uint8_t *stage,
-                                           uint32_t q, uint32_t row0, uint32_t nrows, QuadState &S, int &sp,
-                                           uint32_t (&v)[R], uint32_t &valid) {
-  const uint8_t kind = second ? I.bkind : I.akind;
-  if (kind == OPK_COLUMN) {
-    const DevColumn &c = P.cols[second ? I.bcol : I.acol];
-    if (c.in.mode == 0) {
-#pragma unroll
-      for (int r = 0; r < R; r++) v[r] = (uint32_t)c.in.constLo;
-      valid = c.in.constValid ? 0xF : 0;
-    } else if (STAGED && !c.rle) {
-      fetchStaged(c, stage, q, v, valid);
-    } else {
-      fetchDirect(P, c, row0, nrows, v, valid);
-    }
-  } else if (kind == OPK_CONST) {
-    const uint32_t k = second ? I.bconst : I.aconst;
-#pragma unroll
-    for (int r = 0; r < R; r++) v[r] = k;
-    valid = (second ? I.bvalid : I.avalid) ? 0xF : 0;
-  } else if (kind == OPK_FOREIGN) {
-    // joined dimension table: probe its index with the row's join key, read the foreign column at the RecordID
-    const uint8_t fc = second ? I.bcol : I.acol;
-    const uint8_t t = P.foreignTableOf[fc];
-    const DevColumn &jc = P.cols[P.joinCol[t]];
-    uint32_t key[R], kvalid;
-    if (jc.in.mode == 0) {
-#pragma unroll
-      for (int r = 0; r < R; r++) key[r] = (uint32_t)jc.in.constLo;
-      kvalid = jc.in.constValid ? 0xF : 0;
-    } else if (STAGED) {
-      fetchStaged(jc, stage, q, key, kvalid);
-    } else {
-      fetchDirect(P, jc, row0, nrows, key, kvalid);
-    }
-    valid = 0;
-#pragma unroll
-    for (int r = 0; r < R; r++) {
-      const unsigned long long rid = ((kvalid >> r) & 1) && (uint32_t)r < nrows ? cuckooLookup(P.join->tables[t], key[r], 0) : 0ull;
-      const Cell f = foreignLoad(P.join->cols[fc], rid, nullptr);
-      v[r] = (uint32_t)f.v;
-      valid |= (f.valid ? 1u : 0u) << r;
-    }
-  } else {  // stack pop (static unrolled select keeps the stack in registers)
-    sp--;
-#pragma unroll
-    for (int d = 0; d < ARES_PLAN_STACK_DEPTH; d++) {
-      if (d == sp) {
-#pragma unroll
-        for (int r = 0; r < R; r++) v[r] = S.st[d][r];
-        valid = S.stv[d];
-      }
-    }
-  }
-}
-
-// Processes one quad (rows row0 .. row0+nrows-1 of the batch).
-template <int KW>
-__device__ __forceinline__ void keyInsert(uint64_t (&w)[KW], int byteOff, uint64_t v) {
-  if (KW == 1) {
-    w[0] |= v << ((byteOff & 7) * 8);
-  } else {
-    const int word = byteOff >> 3, sh = (byteOff & 7) * 8;
-#pragma unroll
-    for (int k = 0; k < KW; k++)
-      if (k == word) w[k] |= v << sh;
-  }
-}
 
 // Group key of a packed dimension row: the row itself (KEY_PACKED), or the reference's hash of it.
 __device__ __forceinline__ unsigned long long rowKey(const uint64_t *w, uint8_t keyMode, uint8_t hashBits, int rowBytes) {
   if (keyMode == KEY_PACKED) return w[0];
   return hashBits == 64 ? murmur3_128_lo(w, rowBytes, 0) : (unsigned long long)murmur3_32(w, rowBytes, 0);
-}
-
-template <bool STAGED, bool WIDEKEY>
-__device__ __forceinline__ void processQuad(const DevPlan &P, const DevTable &G, const SmemTable &T, bool useSmem,
-                                            bool allowClaim, const uint8_t *stage, uint32_t q, uint32_t row0,
-                                            uint32_t nrows) {
-  QuadState S;
-  int sp = 0;
-  uint32_t alive = (1u << nrows) - 1u;
-  constexpr int KW = WIDEKEY ? 4 : 1;
-  uint64_t kw[R][KW];
-#pragma unroll
-  for (int r = 0; r < R; r++) {
-#pragma unroll
-    for (int k = 0; k < KW; k++) kw[r][k] = 0;
-  }
-  uint64_t meas[R];
-#pragma unroll
-  for (int r = 0; r < R; r++) meas[r] = P.measureIdentity;
-
-  for (int pc = 0; pc < P.ninsts; pc++) {
-    const DevInst &I = P.insts[pc];
-    if (I.wide) {  // 8/16-byte column copied verbatim into a dimension (Int64 / UUID dims)
-      const DevColumn &c = P.cols[I.acol];
-#pragma unroll
-      for (int r = 0; r < R; r++) {
-        if ((uint32_t)r < nrows) {
-          uint64_t hi = 0;
-          Cell x = loadInput(c.in, row0 + r, nullptr, P.baseCounts, P.startCount, &hi);
-          keyInsert<KW>(kw[r], I.rowOff, x.v);
-          if (I.width == 16) keyInsert<KW>(kw[r], I.rowOff + 8, hi);
-          keyInsert<KW>(kw[r], I.nullOff, x.valid ? 1 : 0);
-        }
-      }
-      continue;
-    }
-    uint32_t a[R], b[R], res[R];
-    uint32_t av = 0, bv = 0, rv = 0;
-    if (I.nops == 2) {
-      // both on the stack: rhs was pushed last
-      if (I.bkind == OPK_STACK) getOperand<STAGED>(P, I, true, stage, q, row0, nrows, S, sp, b, bv);
-      getOperand<STAGED>(P, I, false, stage, q, row0, nrows, S, sp, a, av);
-      if (I.bkind != OPK_STACK) getOperand<STAGED>(P, I, true, stage, q, row0, nrows, S, sp, b, bv);
-      cvtVec(a, (ValClass)I.aclass, (ValClass)I.tclass);
-      cvtVec(b, (ValClass)I.bclass, (ValClass)I.tclass);
-      binVec(I.fn, (ValClass)I.tclass, a, av, b, bv, res, rv);
-    } else {
-      getOperand<STAGED>(P, I, false, stage, q, row0, nrows, S, sp, a, av);
-      unVec(I.fn, (ValClass)I.aclass, a, av, res, rv);
-    }
-    switch (I.sink) {
-      case PLAN_SINK_STACK: {
-        cvtVec(res, (ValClass)I.rclass, (ValClass)I.oclass);
-#pragma unroll
-        for (int d = 0; d < ARES_PLAN_STACK_DEPTH; d++) {
-          if (d == sp) {
-#pragma unroll
-            for (int r = 0; r < R; r++) S.st[d][r] = res[r];
-            S.stv[d] = rv;
-          }
-        }
-        sp++;
-        break;
-      }
-      case PLAN_SINK_FILTER: {
-        uint32_t keep = 0;
-        if (I.rclass == VC_F32) {
-#pragma unroll
-          for (int r = 0; r < R; r++) keep |= (__uint_as_float(res[r]) != 0.0f ? 1u : 0u) << r;
-        } else {
-#pragma unroll
-          for (int r = 0; r < R; r++) keep |= (res[r] != 0 ? 1u : 0u) << r;
-        }
-        alive &= keep;
-        if (pc == P.lastFilter && !__any_sync(__activemask(), alive != 0)) return;
-        break;
-      }
-      case PLAN_SINK_DIMENSION: {
-#pragma unroll
-        for (int r = 0; r < R; r++) {
-          uint64_t o = cvt(res[r], (ValClass)I.rclass, (ValClass)I.oclass);
-          keyInsert<KW>(kw[r], I.rowOff, o);
-          keyInsert<KW>(kw[r], I.nullOff, (rv >> r) & 1);
-        }
-        break;
-      }
-      default: {  // PLAN_SINK_MEASURE
-#pragma unroll
-        for (int r = 0; r < R; r++) {
-          if ((rv >> r) & 1) {
-            uint64_t o = cvt(res[r], (ValClass)I.rclass, (ValClass)I.oclass);
-            if (P.aggOp == OP_AVG) {  // (float average, count) pair, as assignAvg packs it (query/iterator.hpp:636-645)
-              uint32_t cnt = 1;
-              if (P.baseCounts != nullptr && (uint32_t)r < nrows) cnt = P.baseCounts[row0 + r + 1] - P.baseCounts[row0 + r];
-              meas[r] = ((uint64_t)cnt << 32) | (uint32_t)cvt(o, (ValClass)I.oclass, VC_F32);
-              continue;
-            }
-            if (!P.skipCount && P.baseCounts != nullptr && (uint32_t)r < nrows) {
-              uint32_t cnt = P.baseCounts[row0 + r + 1] - P.baseCounts[row0 + r];
-              o = mulCount(o, (ValClass)I.oclass, cnt);
-            }
-            meas[r] = o;
-          }
-        }
-        break;
-      }
-    }
-  }
-
-  if (alive == 0) return;
-  const AggOp op = (AggOp)P.aggOp;
-#pragma unroll
-  for (int r = 0; r < R; r++) {
-    if (!((alive >> r) & 1)) continue;
-    unsigned long long key;
-    const uint64_t *roww = nullptr;
-    if constexpr (WIDEKEY) {
-      key = rowKey(kw[r], KEY_HASHED, P.hashBits, P.rowBytes);
-      if (P.hll == 1) key = (key & 0xFFFFFFFFFFFF0000ull) | (meas[r] & 0x3FFFu);
-      roww = kw[r];
-    } else {
-      key = kw[r][0];
-    }
-    if (P.hll == 2) {  // dense registers (no shared mirror on this generic path)
-      hllDenseUpdate(G, nullptr, key, roww, (uint32_t)meas[r]);
-      continue;
-    }
-    if (!useSmem || !smemUpdate(T, G, op, key, roww, meas[r], allowClaim)) globalUpdate(G, op, key, roww, meas[r]);
-  }
-}
-
-// ---------------------------------------------------------------------------------------
-// the fused kernel
-// ---------------------------------------------------------------------------------------
-__device__ __forceinline__ void issueTile(const DevPlan &P, uint32_t tile, uint8_t *stage, uint64_t *bar) {
-  // one elected thread: arm the barrier with the byte count, then one bulk copy per column part
-  uint32_t total = 0;
-  for (int c = 0; c < P.ncols; c++) {
-    const DevColumn &col = P.cols[c];
-    if (col.staged) total += col.tileValueBytes;
-    if (col.hasNulls) total += col.tileNullBytes;
-  }
-  mbarExpectTx(bar, total);
-  const size_t row0 = (size_t)tile * P.tileRows;
-  for (int c = 0; c < P.ncols; c++) {
-    const DevColumn &col = P.cols[c];
-    if (col.staged) {
-      const uint8_t *src = col.in.base + col.in.valuesOff + (col.width ? row0 * col.width : row0 / 8);
-      tmaLoad1D(stage + col.smemValues, src, col.tileValueBytes, bar);
-    }
-    if (col.hasNulls) {
-      const uint8_t *src = col.in.base + col.in.nullsOff + row0 / 8;
-      tmaLoad1D(stage + col.smemNulls, src, col.tileNullBytes, bar);
-    }
-  }
-}
-
-template <bool WIDEKEY>
-__global__ void __launch_bounds__(kFusedThreads, 1)
-fusedBatchKernel(const __grid_constant__ DevPlan P, const DevTable G) {
-  extern __shared__ __align__(128) uint8_t smem[];
-  uint64_t *bars = reinterpret_cast<uint64_t *>(smem);                       // kStages barriers
-  uint32_t *claims = reinterpret_cast<uint32_t *>(smem + 64);
-  unsigned long long *tKeys = reinterpret_cast<unsigned long long *>(smem + 128);
-  // accumulators of the CTA's table live in an L2-resident private slice of global memory:
-  // fire-and-forget RED instead of shared-memory CAS loops, and 64 KB of shared memory back for the ring
-  unsigned long long *tAcc = P.ctaAcc + (size_t)blockIdx.x * P.smemSlots;
-  uint8_t *stages = reinterpret_cast<uint8_t *>(tKeys + P.smemSlots);
-
-  SmemTable T;
-  T.keys = tKeys; T.acc = tAcc; T.claims = claims; T.mask = P.smemSlots - 1;
-  const bool useSmem = P.smemSlots > 0;
-  for (uint32_t i = threadIdx.x; i < P.smemSlots; i += blockDim.x) {
-    tKeys[i] = kEmptyKey;
-    tAcc[i] = P.accNeutral;
-  }
-  if (threadIdx.x == 0) {
-    *claims = 0;
-    for (int s = 0; s < kMaxStages; s++) mbarInit(&bars[s], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-
-  const uint32_t quadsPerTile = P.tileRows / R;
-  // Growth of the group table (see jit_kernel_tail.cuh): this kernel stops at CTA granularity — thread 0 looks at the
-  // STOP flag before every tile — and records the iterations it has folded; a resumed launch starts there.
-  volatile uint32_t &sStop = *reinterpret_cast<volatile uint32_t *>(smem + 72);   // header word (no static shared memory)
-  const uint32_t progIdx = blockIdx.x * kProgressWarps;
-  uint32_t foldedUntil = 0xFFFFFFFFu;
-  // ---- staged full tiles: tile t handled by CTA (t mod gridDim), ring of kStages buffers ----
-  if (P.staged && P.numFullTiles > 0) {
-    const uint32_t first = blockIdx.x, step = gridDim.x;
-    const uint32_t startIt = P.resume ? G.progress[progIdx] : 0u;
-    if (threadIdx.x == 0 && startIt != 0xFFFFFFFFu) {
-      for (uint32_t s = 0; s < P.numStages; s++) {
-        uint32_t t = first + (startIt + s) * step;
-        if (t < P.numFullTiles) issueTile(P, t, stages + (size_t)s * P.stageBytes, &bars[s]);
-      }
-    }
-    uint32_t it = 0, drainEnd = 0xFFFFFFFFu;
-    bool draining = false;
-    for (uint32_t t = first + startIt * step; startIt != 0xFFFFFFFFu && t < P.numFullTiles && it < drainEnd; t += step, it++) {
-      const uint32_t s = it % P.numStages, parity = (it / P.numStages) & 1;
-      if (!draining) {
-        if (threadIdx.x == 0) sStop = *reinterpret_cast<volatile uint32_t *>(&G.counters[3]);
-        __syncthreads();
-        if (sStop != 0u && P.hll != 2) {   // stop folding; the tiles already in flight are still waited for
-          draining = true;
-          foldedUntil = startIt + it;
-          drainEnd = it + P.numStages;
-        }
-      }
-      mbarWait(&bars[s], parity);
-      if (draining) continue;
-      const uint8_t *stage = stages + (size_t)s * P.stageBytes;
-      // shared-table admission is decided per tile (uniform in the CTA)
-      const bool allowClaim = *reinterpret_cast<volatile uint32_t *>(claims) < (P.smemSlots / 4) * 3;
-      for (uint32_t q = threadIdx.x; q < quadsPerTile; q += blockDim.x)
-        processQuad<true, WIDEKEY>(P, G, T, useSmem, allowClaim, stage, q, t * P.tileRows + q * R, R);
-      __syncthreads();  // everyone is done reading stage s
-      if (threadIdx.x == 0) {
-        uint32_t nt = t + P.numStages * step;
-        if (nt < P.numFullTiles) issueTile(P, nt, stages + (size_t)s * P.stageBytes, &bars[s]);
-      }
-    }
-  }
-  if (threadIdx.x == 0) G.progress[progIdx] = foldedUntil;
-  // ---- rows not covered by staged tiles (tail, or the whole batch on the direct path) --------
-  // (every CTA folds its share of them once: progress[progIdx + 1] says so to a resumed launch; a launch that found the
-  // table at its threshold leaves its share to the next one.  The host makes room for direct-path batches up front.)
-  if (threadIdx.x == 0) {
-    if (!P.resume) G.progress[progIdx + 1] = 0u;
-    sStop = (P.hll != 2 && *reinterpret_cast<volatile uint32_t *>(&G.counters[3]) != 0u) || G.progress[progIdx + 1] != 0u;
-    if (!sStop) G.progress[progIdx + 1] = 1u;
-  }
-  __syncthreads();
-  if (!sStop) {
-    const uint32_t begin = P.staged ? P.numFullTiles * P.tileRows : P.tailBegin;
-    const uint32_t quads = (P.numRows - begin + R - 1) / R;
-    const bool allowClaim = true;
-    for (uint32_t q = blockIdx.x * blockDim.x + threadIdx.x; q < quads; q += gridDim.x * blockDim.x) {
-      uint32_t row0 = begin + q * R;
-      uint32_t nrows = P.numRows - row0 < R ? P.numRows - row0 : R;
-      processQuad<false, WIDEKEY>(P, G, T, useSmem, allowClaim, nullptr, q, row0, nrows);
-    }
-  }
-  // ---- flush the shared table into the global one ---------------------------------------------
-  __syncthreads();
-  if (P.hll == 2) return;
-  const AggOp op = (AggOp)P.aggOp;
-  for (uint32_t i = threadIdx.x; i < P.smemSlots; i += blockDim.x) {
-    unsigned long long k = tKeys[i];
-    if (k != kEmptyKey) globalUpdate(G, op, k, nullptr, __ldcg(&tAcc[i]), /*spillWhenStopped=*/true);
-  }
-  if (blockIdx.x == 0 && threadIdx.x == 0) *G.occPublish = *reinterpret_cast<volatile uint32_t *>(&G.counters[0]);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1481,9 +1000,9 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P) {
 }
 
 // ---------------------------------------------------------------------------------------
-// archive batches: run-length encoded (mode-3) columns are expanded once per batch into plain
-// mode-2 scratch columns (one value + one validity bit per index position), so that the staged,
-// specialised kernel can run on them instead of a positional run search per access per row.
+// archive batches: run-length encoded (mode-3) columns that the kernel does not decode from their runs
+// are expanded once per batch into plain mode-2 scratch columns (one value + one validity bit per
+// index position), see prepareInputs.
 // ---------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 expandRleKernel(InputDesc d, const uint32_t *__restrict__ baseCounts, uint32_t startCount, uint32_t n, int width, bool direct,
@@ -1504,7 +1023,12 @@ expandRleKernel(InputDesc d, const uint32_t *__restrict__ baseCounts, uint32_t s
         case 0: bit = bitAt(vals, p + d.startBit); break;
         case 1: outValues[i] = vals[p]; break;
         case 2: reinterpret_cast<uint16_t *>(outValues)[i] = reinterpret_cast<const uint16_t *>(vals)[p]; break;
-        default: reinterpret_cast<uint32_t *>(outValues)[i] = reinterpret_cast<const uint32_t *>(vals)[p]; break;
+        case 4: reinterpret_cast<uint32_t *>(outValues)[i] = reinterpret_cast<const uint32_t *>(vals)[p]; break;
+        case 8: reinterpret_cast<uint64_t *>(outValues)[i] = reinterpret_cast<const uint64_t *>(vals)[p]; break;
+        default:   // UUID (8-byte aligned, as wide columns are)
+          reinterpret_cast<uint64_t *>(outValues)[2 * (size_t)i] = reinterpret_cast<const uint64_t *>(vals)[2 * (size_t)p];
+          reinterpret_cast<uint64_t *>(outValues)[2 * (size_t)i + 1] = reinterpret_cast<const uint64_t *>(vals)[2 * (size_t)p + 1];
+          break;
       }
     }
     const uint32_t vword = __ballot_sync(0xFFFFFFFFu, valid), bword = __ballot_sync(0xFFFFFFFFu, bit);
@@ -1528,25 +1052,20 @@ rleTileRunsKernel(const uint32_t *__restrict__ counts, uint32_t length, const ui
   out[t] = rlePosition(counts, length, row);
 }
 
-// Decides staged vs direct, the tile size, the stage layout, the TMA ring depth and the shared table
-// size.  The shared table gets what the workload needs first (a table that overflows sends rows to
-// contended L2 atomics, tools/microbench/agg_microbench.cu), the ring takes the rest.
-static size_t layoutStages(DevPlan &P, uint32_t expectedGroups, bool allowDense = true) {
-  bool canStage = P.numRows >= 1024;
+// SUM / AVG need the run lengths of an archive batch, and RLE columns the row numbers of its index positions: the base
+// counts are then staged with the columns.
+static bool stagesBaseCounts(const DevPlan &P) {
+  if (P.baseCounts == nullptr) return false;
   bool anyRle = false;
-  uint32_t rowBits = 0;
-  for (int c = 0; c < P.ncols; c++) {
-    DevColumn &col = P.cols[c];
-    if (col.in.mode == 0 || !col.used) continue;
-    if (col.rle) { anyRle = true; continue; }            // RLE decoded in the kernel from its runs: nothing to stage
-    if (col.in.mode == 3) { canStage = false; break; }  // RLE without the specialised kernel: positional search, direct path
-    if (col.width > 4) continue;                          // wide dims are read directly
-    const uintptr_t v = reinterpret_cast<uintptr_t>(col.in.base + col.in.valuesOff);
-    if (v & 15) canStage = false;
-    if (col.in.mode == 2 && (reinterpret_cast<uintptr_t>(col.in.base + col.in.nullsOff) & 15)) canStage = false;
-    rowBits += col.width ? col.width * 8 : 1;
-    if (col.in.mode == 2) rowBits += 1;
-  }
+  for (int c = 0; c < P.ncols; c++) anyRle = anyRle || (P.cols[c].used && P.cols[c].rle);
+  return !P.skipCount || anyRle;
+}
+
+// Decides the tile size, the stage layout, the TMA ring depth and the shared table size.  The shared table gets what the
+// workload needs first (a table that overflows sends rows to contended L2 atomics, tools/microbench/agg_microbench.cu),
+// the ring takes the rest.  Staged parts must start on a 16-byte boundary (executePlan copies those that do not).
+static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
+  const bool stageBc = stagesBaseCounts(P);
   // The shared table takes 8192 slots (128 KB) whenever a ring of >= 2 stages still fits beside
   // it: measured on cfg3 (2,400 groups per batch) 8192 slots beat 4096 by 1.5x because fewer
   // probe iterations are paid per warp; a plan with very wide rows falls back to fewer slots.
@@ -1556,8 +1075,7 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups, bool allowDense 
   P.bypassOk = (P.hll || expectedGroups > 4 * slots) ? 1 : 0;
   // zone map known for every dimension: no key table, slots addressed by dimension value (jit.cu)
   P.denseGlobal = 0;
-  if (allowDense) jitAnalyzeDense(P, P.bypassOk != 0);
-  else P.denseNd = 0;
+  jitAnalyzeDense(P, P.bypassOk != 0);
   auto stageBytesFor = [&](uint32_t tr) {
     size_t stage = 0;
     for (int c = 0; c < P.ncols; c++) {
@@ -1566,94 +1084,90 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups, bool allowDense 
       stage += ((col.width ? (size_t)tr * col.width : tr / 8 + 16) + 15) / 16 * 16;
       if (col.in.mode == 2) stage += (tr / 8 + 16 + 15) / 16 * 16;
     }
-    // base counts of an RLE batch ride along when a SUM / AVG measure needs the run lengths, or an RLE column the row numbers
-    if (P.baseCounts != nullptr && (!P.skipCount || anyRle) && (reinterpret_cast<uintptr_t>(P.baseCounts) & 15) == 0) stage += ((size_t)tr + 4) * 4;
+    if (stageBc) stage += ((size_t)tr + 4) * 4;
     return stage;
   };
+  // stages of tiles of `tr` rows that fit in `avail` bytes (a plan that stages nothing has empty stages: any number fits)
+  auto stagesIn = [&](size_t avail, uint32_t tr) -> uint32_t {
+    const size_t bytes = stageBytesFor(tr), n = bytes ? avail / bytes : (size_t)kMaxStages;
+    return n > (size_t)kMaxStages ? (uint32_t)kMaxStages : (uint32_t)n;
+  };
+  // keep >= 128 rows for the tail so that the last full tile's 16-byte bitmap over-read stays inside the column
+  auto fullTiles = [&](uint32_t tr) { return P.numRows > 128 ? (P.numRows - 128) / tr : 0u; };
   uint32_t tileRows = 0, stages = 0;
-  if (canStage && rowBits > 0) {
-    if (P.denseNd != 0) {
-      // Dense slots cost 9 bytes each (flag + 8-byte accumulator).  Give the ring as many stages as possible
-      // and the slots the rest: the capacity (part of the kernel text) then depends on the stage layout only,
-      // not on the batch's ranges.
+  if (P.denseNd != 0) {
+    // Dense slots cost 9 bytes each (flag + 8-byte accumulator).  Give the ring as many stages as possible
+    // and the slots the rest: the capacity (part of the kernel text) then depends on the stage layout only,
+    // not on the batch's ranges.
+    for (uint32_t tr : {3968u, 1920u, 896u}) {
+      for (uint32_t n = kMaxStages; n >= 2 && !tileRows; n--) {
+        const size_t need = 128 + n * stageBytesFor(tr);
+        if (need >= (size_t)kSmemBudget) continue;
+        // three 32-bit piece counters, or flag + 8-byte accumulator; HLL: one 32-bit map entry (slot -> group's registers)
+        const size_t slotBytes = P.hll ? 4 : P.denseFx ? 12 : 9;
+        uint32_t cap = (uint32_t)(((size_t)kSmemBudget - need) / slotBytes / 16 * 16);
+        if (cap > kDenseMaxSlots) cap = kDenseMaxSlots;
+        if (cap >= P.denseTotal) { tileRows = tr; stages = n; slots = cap; }
+      }
+      if (tileRows) break;
+    }
+    if (!tileRows && !P.hll && P.neutralSafe && P.denseTotal <= kGlobalDenseMaxSlots) {
+      // more slots than a CTA holds: one accumulator array in global memory for the whole grid; shared memory is all ring
       for (uint32_t tr : {3968u, 1920u, 896u}) {
-        for (uint32_t n = kMaxStages; n >= 2 && !tileRows; n--) {
-          const size_t need = 128 + n * stageBytesFor(tr);
-          if (need >= (size_t)kSmemBudget) continue;
-          // three 32-bit piece counters, or flag + 8-byte accumulator; HLL: one 32-bit map entry (slot -> group's registers)
-          const size_t slotBytes = P.hll ? 4 : P.denseFx ? 12 : 9;
-          uint32_t cap = (uint32_t)(((size_t)kSmemBudget - need) / slotBytes / 16 * 16);
-          if (cap > kDenseMaxSlots) cap = kDenseMaxSlots;
-          if (cap >= P.denseTotal) { tileRows = tr; stages = n; slots = cap; }
+        const uint32_t n = stagesIn((size_t)kSmemBudget - 128 - 256, tr);
+        if (n >= 2) {
+          tileRows = tr; stages = n; slots = 16; P.denseGlobal = 1;
+          // L2 atomics saturate at >= ~1M distinct addresses and contend below (tools/microbench/agg_microbench.cu):
+          // replicate the slot array until it has about that many
+          uint32_t reps = 1;
+          while (reps < 8 && (uint64_t)P.denseTotal * reps * 2 <= kGlobalDenseMaxSlots && (uint64_t)P.denseTotal * reps < (1u << 20)) reps *= 2;
+          P.denseGlobalReps = (uint8_t)reps;
+          break;
         }
-        if (tileRows) break;
-      }
-      if (!tileRows && !P.hll && P.neutralSafe && P.denseTotal <= kGlobalDenseMaxSlots) {
-        // more slots than a CTA holds: one accumulator array in global memory for the whole grid; shared memory is all ring
-        for (uint32_t tr : {3968u, 1920u, 896u}) {
-          const uint32_t n = (uint32_t)(((size_t)kSmemBudget - 128 - 256) / stageBytesFor(tr));
-          if (n >= 2) {
-            tileRows = tr; stages = n > (uint32_t)kMaxStages ? kMaxStages : n; slots = 16; P.denseGlobal = 1;
-            // L2 atomics saturate at >= ~1M distinct addresses and contend below (tools/microbench/agg_microbench.cu):
-            // replicate the slot array until it has about that many
-            uint32_t reps = 1;
-            while (reps < 8 && (uint64_t)P.denseTotal * reps * 2 <= kGlobalDenseMaxSlots && (uint64_t)P.denseTotal * reps < (1u << 20)) reps *= 2;
-            P.denseGlobalReps = (uint8_t)reps;
-            break;
-          }
-        }
-      }
-      if (!tileRows) P.denseNd = 0;   // no layout holds the slots: hash table
-    }
-    if (!tileRows) {
-      for (uint32_t sl : {slots, slots / 2, slots / 4}) {
-        for (uint32_t tr : {3968u, 1920u, 896u}) {  // 128 rows x (31 | 15 | 7) consumer warps
-          size_t avail = (size_t)kSmemBudget - 128 - (size_t)sl * 8;
-          uint32_t n = (uint32_t)(avail / stageBytesFor(tr));
-          if (n >= 2) { tileRows = tr; stages = n > (uint32_t)kMaxStages ? kMaxStages : n; break; }
-        }
-        if (tileRows) { slots = sl; break; }
       }
     }
-  } else {
-    P.denseNd = 0;
+    // no layout holds the slots, or a batch without a full tile (all of it is the tail, which one CTA folds): hash table
+    if (tileRows && fullTiles(tileRows) == 0) { tileRows = 0; slots = 8192; }
+    if (!tileRows) { P.denseNd = 0; P.denseGlobal = 0; }
+  }
+  if (!tileRows) {
+    for (uint32_t sl : {slots, slots / 2, slots / 4}) {
+      for (uint32_t tr : {3968u, 1920u, 896u}) {  // 128 rows x (31 | 15 | 7) consumer warps
+        const uint32_t n = stagesIn((size_t)kSmemBudget - 128 - (size_t)sl * 8, tr);
+        if (n >= 2) { tileRows = tr; stages = n; break; }
+      }
+      if (tileRows) { slots = sl; break; }
+    }
+    // (sixteen 4-byte columns with null bitmaps and the base counts take 62 KB per 896-row stage: two fit beside 8192 slots)
+    if (!tileRows) throw EngineError("no stage layout fits the plan's columns into shared memory");
   }
   size_t stageBytes = 0;
-  bool anyStaged = false;
-  if (tileRows) {
-    for (int c = 0; c < P.ncols; c++) {
-      DevColumn &col = P.cols[c];
-      if (col.in.mode == 0 || !col.used || col.width > 4 || col.rle) continue;
-      col.staged = 1;
-      anyStaged = true;
-      col.smemValues = (uint32_t)stageBytes;
-      // bit-packed bools and bitmaps copy one 16-byte chunk beyond the tile so that a non-zero
-      // StartingIndex can read across the tile's last byte; full tiles always have those bytes.
-      col.tileValueBytes = col.width ? tileRows * col.width : tileRows / 8 + 16;
-      stageBytes += (col.tileValueBytes + 15) / 16 * 16;
-      if (col.in.mode == 2) {
-        col.hasNulls = 1;
-        col.smemNulls = (uint32_t)stageBytes;
-        col.tileNullBytes = tileRows / 8 + 16;
-        stageBytes += (col.tileNullBytes + 15) / 16 * 16;
-      }
+  for (int c = 0; c < P.ncols; c++) {
+    DevColumn &col = P.cols[c];
+    if (col.in.mode == 0 || !col.used || col.width > 4 || col.rle) continue;
+    col.staged = 1;
+    col.smemValues = (uint32_t)stageBytes;
+    // bit-packed bools and bitmaps copy one 16-byte chunk beyond the tile so that a non-zero
+    // StartingIndex can read across the tile's last byte; full tiles always have those bytes.
+    col.tileValueBytes = col.width ? tileRows * col.width : tileRows / 8 + 16;
+    stageBytes += (col.tileValueBytes + 15) / 16 * 16;
+    if (col.in.mode == 2) {
+      col.hasNulls = 1;
+      col.smemNulls = (uint32_t)stageBytes;
+      col.tileNullBytes = tileRows / 8 + 16;
+      stageBytes += (col.tileNullBytes + 15) / 16 * 16;
     }
   }
   P.smemBc = 0;
   P.tileBcBytes = 0;
-  if (anyStaged && P.baseCounts != nullptr && (!P.skipCount || anyRle) && (reinterpret_cast<uintptr_t>(P.baseCounts) & 15) == 0) {
+  if (stageBc) {
     P.smemBc = (uint32_t)stageBytes;
     P.tileBcBytes = (tileRows + 4) * 4;   // one count more than rows (run length = difference), padded to 16 bytes
     stageBytes += P.tileBcBytes;
   }
-  P.staged = anyStaged;
-  P.tileRows = anyStaged ? tileRows : 4 * kFusedThreads;
-  P.numStages = anyStaged ? stages : 0;
-  // keep >= 128 rows for the direct tail so that the last staged tile's 16-byte bitmap over-read
-  // stays inside the column
-  P.numFullTiles = anyStaged && P.numRows > 128 ? (P.numRows - 128) / tileRows : 0;
-  if (P.numFullTiles == 0) { P.staged = 0; stageBytes = 0; P.numStages = 0; P.denseNd = 0; P.denseGlobal = 0; if (slots > 8192 || slots < 256) slots = 8192; }
-  if (P.denseNd == 0) P.denseGlobal = 0;
+  P.tileRows = tileRows;
+  P.numStages = stages;
+  P.numFullTiles = fullTiles(tileRows);
   P.stageBytes = (uint32_t)stageBytes;
   P.smemSlots = slots;
   P.tableBytes = P.denseNd != 0 ? (slots * (P.hll ? 4 : P.denseFx ? 12 : 9) + 127) / 128 * 128 : slots * 8;
@@ -1776,62 +1290,90 @@ static void ensureRoom(AggState *st, uint64_t bound, cudaStream_t s) {
   st->occUpper += bound;
 }
 
-static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
-  if (bp.NumRows == 0) return;
-  if (bp.NumRows > 0x7FFFFFFFu) throw EngineError("a batch holds at most 2^31-1 rows");
-  static thread_local DevPlan P;  // ~3 KB; passed by value as a __grid_constant__ parameter
-  compilePlan(st, bp, P);
-  P.tailBegin = 0;
-  P.resume = 0;
-  // Archive batches: run-length encoded (mode 3) columns.
-  //  * the column whose count vector IS the batch's base counts has one value per index position: it is read like an
-  //    uncompressed column (values / null bitmap of its runs), no copy;
-  //  * every other RLE column is a FIRST-CLASS input of the specialised kernel: decoded from its runs inside the tile loop
-  //    (jit_kernel_head.cuh ldrle) with a per-tile run hint computed below — HBM sees the runs, not the rows;
-  //  * without NVRTC the column is expanded once per batch for the interpreter.
-  std::vector<std::unique_ptr<Scratch>> expanded;
-  if (bp.NumRows >= 1024) {
-    const uint32_t n = bp.NumRows;
-    // (the tile loop is driven by the TMA ring: at least one plain column must be staged for the RLE columns to ride along)
-    int stageable = 0;
-    for (int c = 0; c < P.ncols; c++) {
-      const DevColumn &col = P.cols[c];
-      if (col.used && col.width <= 4 && (col.in.mode == 1 || col.in.mode == 2)) stageable++;
-      if (col.used && col.in.mode == 3 && col.width <= 4 && bp.BaseCounts != nullptr &&
-          reinterpret_cast<const uint32_t *>(col.in.base) == bp.BaseCounts && col.in.length >= n) stageable++;
+// Makes every input of the plan readable by the kernel as it is (before layoutStages).
+// Archive batches: run-length encoded (mode 3) columns.
+//  * the column whose count vector IS the batch's base counts has one value per index position: it is read like an
+//    uncompressed column (values / null bitmap of its runs), no copy;
+//  * up to kJitMaxRle other 1- to 4-byte RLE columns are FIRST-CLASS inputs of the kernel: decoded from their runs inside
+//    the tile loop (jit_kernel_head.cuh ldrle) with a per-tile run hint computed by executePlan — HBM sees the runs, not
+//    the rows;
+//  * the others (and 8- / 16-byte ones, which the kernel reads row by row) are expanded once per batch into mode-2
+//    scratch columns (one value + one validity bit per index position).
+// Staged parts (values and null bitmaps of 1- to 4-byte columns, the base counts) are fetched by the TMA engine, which
+// needs a 16-byte aligned source: a part that is not aligned is copied once, byte for byte (same bit offset).
+// `scratch` == nullptr (AresJitDryRun, no device memory): descriptors are rewritten as if, nothing is allocated, copied
+// or launched — the kernel text does not depend on addresses.
+static void prepareInputs(DevPlan &P, const BatchPlan &bp, cudaStream_t s, std::vector<std::unique_ptr<Scratch>> *scratch) {
+  const uint32_t n = P.numRows;
+  auto alloc = [&](size_t bytes) -> uint8_t * {
+    if (scratch == nullptr) return nullptr;
+    scratch->emplace_back(new Scratch(bytes, s));
+    return scratch->back()->as<uint8_t>();
+  };
+  int nrle = 0;
+  for (int c = 0; c < P.ncols; c++) {
+    DevColumn &col = P.cols[c];
+    if (!col.used || col.in.mode != 3) continue;
+    const bool direct = bp.BaseCounts != nullptr && reinterpret_cast<const uint32_t *>(col.in.base) == bp.BaseCounts;
+    if (direct && col.in.length >= n) {   // run number == index position
+      col.in.mode = 2;
+      continue;
     }
-    const bool firstClass = jitAvailable() && stageable > 0;
-    int nrle = 0;
-    for (int c = 0; c < P.ncols; c++) {
-      DevColumn &col = P.cols[c];
-      if (!col.used || col.in.mode != 3 || col.width > 4) continue;
-      const bool direct = bp.BaseCounts != nullptr && reinterpret_cast<const uint32_t *>(col.in.base) == bp.BaseCounts;
-      if (direct && col.in.length >= n) {   // run number == index position
-        col.in.mode = 2;
-        continue;
-      }
-      if (firstClass && nrle < 4 && col.in.length > 0) {
-        col.rle = 1;
-        nrle++;
-        continue;
-      }
-      const size_t nullBytes = ((size_t)(n + 31) / 32 * 4 + 16 + 63) / 64 * 64;
-      const size_t valueBytes = (col.width ? (size_t)n * col.width : (size_t)(n + 31) / 32 * 4) + 64;
-      expanded.emplace_back(new Scratch(nullBytes + valueBytes, s));
-      uint8_t *buf = expanded.back()->as<uint8_t>();
+    if (col.width <= 4 && nrle < kJitMaxRle && col.in.length > 0) {
+      col.rle = 1;
+      nrle++;
+      continue;
+    }
+    const size_t nullBytes = ((size_t)(n + 31) / 32 * 4 + 16 + 63) / 64 * 64;
+    const size_t valueBytes = (col.width ? (size_t)n * col.width : (size_t)(n + 31) / 32 * 4) + 64;
+    uint8_t *buf = alloc(nullBytes + valueBytes);
+    if (buf != nullptr) {
       int blocks = divUp((int64_t)(n + 31) / 32, 8);
       if (blocks > smCount() * 16) blocks = smCount() * 16;
       expandRleKernel<<<blocks, 256, 0, s>>>(col.in, bp.BaseCounts, bp.StartCount, n, col.width, direct, buf + nullBytes,
                                              reinterpret_cast<uint32_t *>(buf));
       checkLastError("expandRle");
-      col.in.base = buf;
-      col.in.nullsOff = 0;
-      col.in.valuesOff = (uint32_t)nullBytes;
-      col.in.length = n;
-      col.in.mode = 2;
-      col.in.startBit = 0;
     }
+    col.in.base = buf;
+    col.in.nullsOff = 0;
+    col.in.valuesOff = (uint32_t)nullBytes;
+    col.in.length = n;
+    col.in.mode = 2;
+    col.in.startBit = 0;
   }
+  if (scratch == nullptr) return;
+  auto misaligned = [](const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; };
+  for (int c = 0; c < P.ncols; c++) {
+    DevColumn &col = P.cols[c];
+    if (!col.used || col.rle || col.width > 4 || (col.in.mode != 1 && col.in.mode != 2)) continue;
+    const uint8_t *values = col.in.base + col.in.valuesOff, *nulls = col.in.base + col.in.nullsOff;
+    const bool hasNulls = col.in.mode == 2;
+    if (!misaligned(values) && !(hasNulls && misaligned(nulls))) continue;
+    // (the kernel reads the bytes of the batch's rows: a full tile's 16-byte bitmap over-read stays below row numRows - 1)
+    const size_t bitBytes = ((size_t)n + col.in.startBit + 7) / 8;
+    const size_t valueBytes = col.width ? (size_t)n * col.width : bitBytes, nullBytes = hasNulls ? (bitBytes + 15) / 16 * 16 : 0;
+    uint8_t *buf = alloc(nullBytes + valueBytes);
+    if (hasNulls) ARES_CUDA(cudaMemcpyAsync(buf, nulls, bitBytes, cudaMemcpyDefault, s));
+    ARES_CUDA(cudaMemcpyAsync(buf + nullBytes, values, valueBytes, cudaMemcpyDefault, s));
+    col.in.base = buf;
+    col.in.nullsOff = 0;
+    col.in.valuesOff = (uint32_t)nullBytes;
+  }
+  if (stagesBaseCounts(P) && misaligned(P.baseCounts)) {
+    uint8_t *buf = alloc(((size_t)n + 1) * 4);
+    ARES_CUDA(cudaMemcpyAsync(buf, P.baseCounts, ((size_t)n + 1) * 4, cudaMemcpyDefault, s));
+    P.baseCounts = reinterpret_cast<const uint32_t *>(buf);
+  }
+}
+
+static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
+  if (bp.NumRows == 0) return;
+  if (bp.NumRows > 0x7FFFFFFFu) throw EngineError("a batch holds at most 2^31-1 rows");
+  static thread_local DevPlan P;  // ~3 KB
+  compilePlan(st, bp, P);
+  P.resume = 0;
+  std::vector<std::unique_ptr<Scratch>> scratch;   // expanded / realigned columns, run hints: released in stream order
+  prepareInputs(P, bp, s, &scratch);
   // joined dimension tables: indexes + foreign-column batches go to device memory for the kernel's lifetime
   std::unique_ptr<Scratch> joinMem;
   P.join = nullptr;
@@ -1857,33 +1399,22 @@ static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
   for (int c = 0; c < P.ncols; c++) {
     DevColumn &col = P.cols[c];
     if (!col.rle) continue;
-    if (!P.staged) { col.rle = 0; continue; }   // no tile loop (tiny batch): the generic positional read
     const uint32_t entries = (P.numRows + P.tileRows - 1) / P.tileRows + 2;
-    expanded.emplace_back(new Scratch(sizeof(uint32_t) * entries, s));
+    scratch.emplace_back(new Scratch(sizeof(uint32_t) * entries, s));
     rleTileRunsKernel<<<divUp(entries, 256), 256, 0, s>>>(reinterpret_cast<const uint32_t *>(col.in.base), col.in.length, bp.BaseCounts,
-                                                         bp.StartCount, P.numRows, P.tileRows, entries, expanded.back()->as<uint32_t>());
+                                                         bp.StartCount, P.numRows, P.tileRows, entries, scratch.back()->as<uint32_t>());
     checkLastError("rleTileRuns");
-    col.tileRun = expanded.back()->as<uint32_t>();
+    col.tileRun = scratch.back()->as<uint32_t>();
   }
-  // room in the group table (see "growth of the group table"): the direct path and the direct-indexed kernels are not
-  // waited for, so what they may insert is reserved up front (flush of the CTA slots / fold of the global slot array;
-  // out-of-range rows park); hash-table tile kernels are checked after the launch and resumed when they stopped.
-  const bool resumable = P.staged && P.denseNd == 0 && !st->hllDense;
-  if (!resumable && !st->hllDense) ensureRoom(st, P.staged ? (uint64_t)P.denseTotal : (uint64_t)P.numRows, s);
+  // room in the group table (see "growth of the group table"): the direct-indexed kernels are not waited for, so what
+  // they may insert is reserved up front (flush of the CTA slots / fold of the global slot array; out-of-range rows
+  // park); hash-table kernels are checked after the launch and resumed when they stopped.
+  const bool resumable = P.denseNd == 0 && !st->hllDense;
+  if (!resumable && !st->hllDense) ensureRoom(st, (uint64_t)P.denseTotal, s);
   P.ctaAcc = st->ctaAcc;   // (after a possible growth: the slices live in the table's allocation)
-  static bool attrSet[64] = {false};
-  if (!attrSet[st->device & 63]) {
-    ARES_CUDA(cudaFuncSetAttribute(fusedBatchKernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget));
-    ARES_CUDA(cudaFuncSetAttribute(fusedBatchKernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget));
-    attrSet[st->device & 63] = true;
-  }
-  auto gridFor = [&]() {
-    int g = smCount() < kMaxGridCtas ? smCount() : kMaxGridCtas;
-    const uint32_t work = P.staged ? P.numFullTiles : (P.numRows + 4 * kFusedThreads - 1) / (4 * kFusedThreads);
-    if ((uint32_t)g > work) g = work ? (int)work : 1;
-    return g;
-  };
-  int grid = gridFor();
+  // one CTA per SM, or per full tile when there are fewer; a batch without a full tile is the tail of one CTA
+  int grid = smCount() < kMaxGridCtas ? smCount() : kMaxGridCtas;
+  if ((uint32_t)grid > P.numFullTiles) grid = P.numFullTiles ? (int)P.numFullTiles : 1;
   if (P.denseGlobal) {
     if (!st->denseAcc) {   // first use: 16 MB of accumulators at the neutral element (denseFoldKernel leaves them so)
       st->denseAcc = static_cast<unsigned long long *>(deviceAllocOrThrow((size_t)kGlobalDenseMaxSlots * sizeof(unsigned long long)));
@@ -1892,41 +1423,27 @@ static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
     }
     P.denseAcc = st->denseAcc;
   }
-  // the specialised kernel covers the staged tiles AND the tail; the interpreter below is the
-  // generic fallback (unaligned / RLE columns, NVRTC unavailable or disabled)
   for (;;) {
-    bool checkAfter = false;   // a hash-table tile kernel ran: wait for it and resume it if the table stopped it
-    if (P.staged && jitLaunchStaged(P, st->table, smemBytes, grid, s)) {
-      checkAfter = P.denseNd == 0 && !st->hllDense;
-      if (P.denseGlobal) {
-        DenseFold F;
-        memset(&F, 0, sizeof(F));
-        uint32_t stride = 1;
-        for (int k = 0; k < P.denseNd; k++) {
-          const DevInst &I = P.insts[P.denseInst[k]];
-          F.lo[k] = P.denseLo[k]; F.cnt[k] = P.denseCnt[k]; F.step[k] = P.denseStep[k]; F.stride[k] = stride;
-          F.rowOff[k] = I.rowOff; F.width[k] = I.width; F.nullOff[k] = I.nullOff;
-          stride *= P.denseCnt[k] + 1;
-        }
-        F.nd = P.denseNd; F.total = P.denseTotal; F.reps = P.denseGlobalReps ? P.denseGlobalReps : 1;
-        F.keyMode = P.keyMode; F.hashBits = P.hashBits; F.rowBytes = P.rowBytes; F.op = P.aggOp;
-        F.neutral = P.accNeutral;
-        int blocks = divUp((int64_t)P.denseTotal, 256);
-        if (blocks > smCount() * 8) blocks = smCount() * 8;
-        denseFoldKernel<<<blocks, 256, 0, s>>>(st->denseAcc, F, st->table);
-        checkLastError("denseFold");
+    jitLaunch(P, st->table, smemBytes, grid, s);
+    if (P.denseGlobal) {
+      DenseFold F;
+      memset(&F, 0, sizeof(F));
+      uint32_t stride = 1;
+      for (int k = 0; k < P.denseNd; k++) {
+        const DevInst &I = P.insts[P.denseInst[k]];
+        F.lo[k] = P.denseLo[k]; F.cnt[k] = P.denseCnt[k]; F.step[k] = P.denseStep[k]; F.stride[k] = stride;
+        F.rowOff[k] = I.rowOff; F.width[k] = I.width; F.nullOff[k] = I.nullOff;
+        stride *= P.denseCnt[k] + 1;
       }
-    } else {
-      if (P.denseNd != 0) {  // the interpreter needs the key-table layout
-        smemBytes = layoutStages(P, st->spec.ExpectedGroups, /*allowDense=*/false);
-        grid = gridFor();
-      }
-      checkAfter = P.staged && !st->hllDense;
-      if (st->keyMode == KEY_HASHED) fusedBatchKernel<true><<<grid, kFusedThreads, smemBytes, s>>>(P, st->table);
-      else fusedBatchKernel<false><<<grid, kFusedThreads, smemBytes, s>>>(P, st->table);
-      checkLastError("ExecuteBatchPlan");
+      F.nd = P.denseNd; F.total = P.denseTotal; F.reps = P.denseGlobalReps ? P.denseGlobalReps : 1;
+      F.keyMode = P.keyMode; F.hashBits = P.hashBits; F.rowBytes = P.rowBytes; F.op = P.aggOp;
+      F.neutral = P.accNeutral;
+      int blocks = divUp((int64_t)P.denseTotal, 256);
+      if (blocks > smCount() * 8) blocks = smCount() * 8;
+      denseFoldKernel<<<blocks, 256, 0, s>>>(st->denseAcc, F, st->table);
+      checkLastError("denseFold");
     }
-    if (!checkAfter) return;
+    if (!resumable) return;   // a hash-table kernel ran: wait for it and resume it if the table stopped it
     // Waiting for every hash-table batch would cost a launch gap per batch (the host cannot prepare the next one while it
     // waits).  The wait is therefore adaptive: always for the first batch of a query, and from then on whenever the
     // occupancy last seen — read back then, or published by a finishing kernel into mapped pinned memory — is above an
@@ -2409,8 +1926,8 @@ CGoCallResHandle AggStateReset(void *state, void *cudaStream, int device) {
 }
 
 // Additive diagnostics, usable without a GPU: generates + NVRTC-compiles the specialised kernel of
-// (spec, plan) and returns the cubin size in res (0: plan not eligible); *sourceOut (optional) gets a
-// malloc'd copy of the generated shape-specific source.
+// (spec, plan) and returns the cubin size in res; *sourceOut (optional) gets a malloc'd copy of the
+// generated shape-specific source.
 CGoCallResHandle AresJitDryRun(AggSpec spec, const BatchPlan *plan, char **sourceOut) {
   CGoCallResHandle h = {nullptr, nullptr};
   try {
@@ -2420,10 +1937,10 @@ CGoCallResHandle AresJitDryRun(AggSpec spec, const BatchPlan *plan, char **sourc
     st.capacity = st.hllDense ? kHllDenseSlots : 0;
     static thread_local DevPlan P;
     compilePlan(&st, *plan, P);
-    P.tailBegin = 0;
+    prepareInputs(P, *plan, nullptr, nullptr);
     layoutStages(P, spec.ExpectedGroups);
     std::string src;
-    size_t n = P.staged ? jitCompileOnly(P, &src) : 0;
+    size_t n = jitCompileOnly(P, &src);
     if (sourceOut) *sourceOut = strdup(src.c_str());
     h.res = reinterpret_cast<void *>(n);
   } catch (const std::exception &e) {

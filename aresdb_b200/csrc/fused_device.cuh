@@ -1,6 +1,6 @@
-// fused_device.cuh — device building blocks shared by the ahead-of-time interpreter kernel
-// (batch_plan.cu) and the NVRTC-specialised kernels (jit.cu): TMA bulk copies + mbarriers, the
-// CTA-private shared-memory group table and the global (L2-resident) group table.
+// fused_device.cuh — device building blocks of the NVRTC-specialised fused kernel (jit.cu) and of
+// the merge / finalize kernels (batch_plan.cu): TMA bulk copies + mbarriers, the CTA-private
+// shared-memory group table and the global (L2-resident) group table.
 // NVRTC-clean: no host headers (the JIT prelude provides the fixed-width typedefs).
 #pragma once
 #include "agg.cuh"

@@ -1,63 +1,12 @@
-// jit_kernel_head.cuh — first half of the NVRTC-specialised fused kernel's source text: runtime
-// parameter block and the quad loaders.  Compiled ONLY by NVRTC (see jit.cu); the generated
+// jit_kernel_head.cuh — first half of the NVRTC-specialised fused kernel's source text: the quad
+// loaders (the runtime parameter block JitParams precedes them: jit_params.cuh).  Compiled ONLY by
+// NVRTC (see jit.cu); the generated
 // rowEval() for one plan shape is pasted between this file and jit_kernel_tail.cuh, after a
 // block of #defines / constexpr tables describing the shape (tile size, stage layout, key words,
 // aggregate op).  Everything shape-dependent is a compile-time constant; only pointers, literal
 // operands and row counts are runtime values, so one compiled kernel serves every batch and every
 // query with the same structure.
 namespace aresb {
-
-constexpr int kJitMaxParts = 32;
-constexpr int kJitMaxConsts = 64;
-constexpr int kJitMaxWide = 8;
-constexpr int kJitMaxMagic = 16;
-constexpr int kJitMaxDenseDims = 8;
-constexpr int kJitMaxRle = 4;
-// A mode-3 column read by the kernel straight from its runs: cumulative counts (length + 1 entries), null bitmap and
-// values of the RUNS, and the per-tile run hint computed by rleTileRunsKernel.
-struct RleColumn {
-  const uint32_t *counts;
-  const uint8_t *nulls, *values;
-  const uint32_t *tileRun;
-  uint32_t length, startBit;
-};
-
-// mirrors plan_device.cuh
-constexpr int kMaxForeignTables = 4;
-constexpr int kMaxForeignCols = 8;
-struct DevJoin {
-  CuckooDesc tables[kMaxForeignTables];
-  ForeignDesc cols[kMaxForeignCols];
-};
-
-struct JitParams {
-  const uint8_t *partSrc[kJitMaxParts];   // global base address of every staged part
-  const uint8_t *wideValues[kJitMaxWide]; // 8/16-byte dimension columns read straight from global
-  const uint8_t *wideNulls[kJitMaxWide];
-  uint32_t consts[kJitMaxConsts];         // literal operands / mode-0 defaults (raw 32-bit cells)
-  unsigned long long magic[kJitMaxMagic]; // 2^64/d + 1 for literal divisors d >= 2 (0: use the generic path)
-  unsigned long long measureIdentity;
-  unsigned long long accNeutral;
-  DevTable G;
-  unsigned long long *ctaAcc;             // [grid][JIT_SMEM_SLOTS] accumulator slices in global memory
-  uint32_t numFullTiles;
-  uint32_t numRows;                       // rows of the batch (tail = numRows - numFullTiles * JIT_TILE_ROWS)
-  // direct-indexed aggregation (JIT_DENSE): dimension k of a row has index (value or quotient) - dLo[k], valid when
-  // below dCnt[k]; index dCnt[k] is the dimension's NULL; slot = sum_k index_k * dStride[k]; value = (dLo + index) * dStep
-  uint32_t dLo[kJitMaxDenseDims], dCnt[kJitMaxDenseDims], dStride[kJitMaxDenseDims], dStep[kJitMaxDenseDims];
-  uint32_t dBase[kJitMaxDenseDims], dSpan[kJitMaxDenseDims], dMagic32[kJitMaxDenseDims];   // span division (see plan_device.cuh)
-  uint32_t dStrideB[kJitMaxDenseDims];   // dStride in the unit the fast path addresses slots in (bytes for the integer form: x 12)
-  uint32_t dTotal, dReps, dRepStride;     // slots of one copy; lane-private copies (power of two), dRepStride slots apart
-  unsigned long long *gAcc;               // JIT_DENSE == 2: the state's global accumulator array (dTotal slots in use)
-  double fxInv;                           // JIT_DENSE_ACC == 4: 2^-S
-  float fxScale;                          //                     2^S (a float sum's rows are added as integers x * 2^S)
-  uint32_t fxPad;
-  const DevJoin *join;                    // joined dimension tables (join.cuh), null without joins
-  uint32_t resume;                        // 1: second launch of the same batch after the table grew (progress[] says where)
-  uint32_t startCount;                    // row number of index position 0 when the batch has no base counts
-  RleColumn rle[kJitMaxRle];              // run-length encoded columns decoded in place (see ldrle)
-};
-
 
 // rows 4q .. 4q+3 of a staged value column of W bytes per value
 template <int W, bool SIGNED>

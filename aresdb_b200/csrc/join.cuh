@@ -1,5 +1,5 @@
 // join.cuh — dimension-table join building blocks (SURVEY.md §8 f4), shared by the legacy HashLookup / ForeignColumnInput
-// entry points, the interpreter kernel and the NVRTC-specialised kernels (NVRTC-clean: no host headers).
+// entry points and the NVRTC-specialised fused kernel (NVRTC-clean: no host headers).
 //
 //   cuckooLookup   probe of the memstore's primary-key index of a dimension table (reference HashLookupFunctor,
 //                  query/functor.hpp:1173-1266; index built by memstore/cuckoo_index.go): numHashes candidate buckets

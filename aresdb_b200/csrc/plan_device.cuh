@@ -1,32 +1,25 @@
 // plan_device.cuh — the device form of a BatchPlan: what compilePlan() (batch_plan.cu) produces and
-// both executors of the staged path consume (the interpreter kernel and the NVRTC generator).
+// the NVRTC generator (jit.cu) specialises the fused kernel for.
 #pragma once
 #include "column.cuh"
 #include "fused_device.cuh"
+#include "jit_params.cuh"
 #include "join.cuh"
 
 namespace aresb {
 
-constexpr int kFusedThreads = 512;
-constexpr int kMaxPlanCols = 16;
 constexpr int kSmemBudget = 232448;           // 227 KB: the most dynamic shared memory a CTA may opt into on sm_90
 constexpr int kJitThreads = 1024;
 constexpr int kMaxGridCtas = 160;             // persistent grid: one CTA per SM (132 on H100 SXM)
+static_assert(kMaxPlanInsts == ARES_MAX_PLAN_INSTS && kMaxForeignTables == ARES_MAX_FOREIGN_TABLES &&
+              kMaxForeignCols == ARES_MAX_FOREIGN_COLUMNS, "jit_params.cuh restates the plan bounds of batch_plan.h");
 
 enum KeyMode : uint8_t { KEY_PACKED = 0, KEY_HASHED = 1 };
 enum OperandKind : uint8_t { OPK_NONE = 0, OPK_COLUMN = 1, OPK_CONST = 2, OPK_STACK = 3, OPK_FOREIGN = 4 };
 
-// Joined dimension tables of a plan, in device memory for the duration of the batch's kernel (uploaded by executePlan).
-constexpr int kMaxForeignTables = ARES_MAX_FOREIGN_TABLES;
-constexpr int kMaxForeignCols = ARES_MAX_FOREIGN_COLUMNS;
-struct DevJoin {
-  CuckooDesc tables[kMaxForeignTables];
-  ForeignDesc cols[kMaxForeignCols];
-};
-
 struct DevColumn {
   InputDesc in;            // how to read it straight from global memory (any mode)
-  uint32_t smemValues;     // byte offsets inside one stage (staged path)
+  uint32_t smemValues;     // byte offsets inside one stage
   uint32_t smemNulls;
   uint32_t tileValueBytes; // bytes of one full tile
   uint32_t tileNullBytes;
@@ -61,10 +54,9 @@ struct DevPlan {
   uint32_t startCount;
   uint32_t numRows;
   uint32_t tileRows;
-  uint32_t numFullTiles;   // staged tiles; the tail goes through the direct path
+  uint32_t numFullTiles;   // staged tiles; the tail (fewer than tileRows + 128 rows) is copied by the kernel itself
   uint32_t stageBytes;
   uint32_t smemSlots;      // shared table slots (power of two)
-  uint32_t tailBegin;      // first row of the direct (non-staged) pass
   uint32_t numStages;      // depth of the TMA ring (2..kMaxStages)
   uint32_t denseSlots;     // dense HLL mode: slots of the group directory (0 otherwise)
   uint32_t smemBc;         // staged base counts (RLE batches, SUM / AVG): byte offset inside a stage, tileBcBytes bytes
@@ -74,7 +66,7 @@ struct DevPlan {
   uint64_t accNeutral;       // neutral element of the combine op
   uint8_t keyMode, rowBytes, valueBytes, hashBits;
   uint8_t aggOp, measWidth, measClass, skipCount;
-  uint8_t hasMeasure, staged, hll, bypassOk;
+  uint8_t hasMeasure, hll, bypassOk;
   // direct-indexed aggregation (jitAnalyzeDense; denseNd == 0: hash table).  Dimension k is produced by instruction
   // denseInst[k]; its slot index is (quotient or value) - denseLo[k], below denseCnt[k]; index denseCnt[k] = NULL.
   uint8_t denseNd;
@@ -108,12 +100,11 @@ constexpr uint32_t kDenseMaxSlots = 8192;   // = slots of a CTA's accumulator sl
 constexpr uint32_t kFxMaxRowsPerCta = 1u << 21;   // each 32-bit piece accumulator takes 2^21 adds of an 11-bit piece
 constexpr uint32_t kGlobalDenseMaxSlots = 1u << 21;   // 16 MB of accumulators per state, allocated on first use
 
-// jit.cu: runs the staged tiles of `P` with a kernel specialised for the plan's shape.  Returns false
-// when NVRTC is unavailable or disabled (ARESDB_B200_JIT=0) so that the caller falls back to the
-// interpreter kernel; throws EngineError when code generation / compilation fails.
-bool jitAvailable();
+// jit.cu: the fused kernel specialised for the plan's shape.  jitLaunch runs a batch on it and throws EngineError when
+// the kernel cannot be built (libnvrtc missing, the shape's compile failed: reported again for every batch of that
+// shape without compiling it twice); jitCompileOnly generates and compiles it without a GPU (AresJitDryRun).
 void jitAnalyzeDense(DevPlan &P, bool bypass);
 size_t jitCompileOnly(const DevPlan &P, std::string *sourceOut);
-bool jitLaunchStaged(const DevPlan &P, const DevTable &G, size_t smemBytes, int grid, cudaStream_t s);
+void jitLaunch(const DevPlan &P, const DevTable &G, size_t smemBytes, int grid, cudaStream_t s);
 
 }  // namespace aresb

@@ -149,24 +149,13 @@ def test_join_sequence_on_b200(name, host_batches):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("jit", ["1", "0"])
+@pytest.mark.parametrize("batches", ["tiles", "tail"])
 @pytest.mark.parametrize("name", ["by_region", "local_hour", "sum_surge", "unmatched"])
-def test_fused_join_on_b200(name, jit, host_batches, monkeypatch):
-    """ExecuteBatchPlan with joined tables (the lookup is a gather stage of the fused kernel; jit=0: the interpreter
-    kernel — the switch is read once per process, so that variant runs in a child) == the reference call sequence."""
-    eng, orc = H.get_backend("b200"), H.get_backend("oracle")
-    if jit == "0":
-        import os
-        import subprocess
-        import sys
-        code = ("import sys; sys.path.insert(0, %r); sys.path.insert(0, %r)\n"
-                "import test_joins as TJ, harness as H, test_pipeline_parity as T\n"
-                "from aresdb_b200 import synth\n"
-                "hbs = [synth.generate_batch(d, n, num_cities=80, null_rate=0.03) for d, n in ((0, 20000), (1, 7777))]\n"
-                "TJ._fused_vs_oracle(%r, hbs)\nprint('ok')\n") % (str(Path(__file__).parent), str(Path(__file__).parent.parent), name)
-        r = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, ARESDB_B200_JIT="0"), capture_output=True, text=True, timeout=600)
-        assert r.returncode == 0 and r.stdout.strip().endswith("ok"), r.stdout[-1500:] + r.stderr[-3000:]
-        return
+def test_fused_join_on_b200(name, batches, host_batches):
+    """ExecuteBatchPlan with joined tables (the lookup is a gather stage of the fused kernel) == the reference call
+    sequence; `tail`: batches without a full tile, whose rows one CTA copies and folds as the tail of its launch."""
+    if batches == "tail":
+        host_batches = [synth.generate_batch(d, n, num_cities=80, null_rate=0.03) for d, n in ((0, 3000), (1, 129))]
     _fused_vs_oracle(name, host_batches)
 
 

@@ -243,8 +243,8 @@ def test_zone_map_integer_accumulation_of_float_sums():
 @pytest.mark.gpu
 def test_zone_map_wide_rows_and_small_batches():
     """Dimension rows wider than 8 bytes are keyed by the reference hash of the packed row: the slots' flush
-    (CTA form) and denseFoldKernel (global form) must rebuild exactly those bytes.  Batches too small to be staged
-    ignore the zone map."""
+    (CTA form) and denseFoldKernel (global form) must rebuild exactly those bytes.  Batches without a full tile
+    ignore the zone map (hash-table form)."""
     eng, orc = H.get_backend("b200"), H.get_backend("oracle")
     hbs = [synth.generate_batch(d, 20011, num_cities=12, null_rate=0.03) for d in range(2)]
     zms = [synth.zone_map(hb) for hb in hbs]
