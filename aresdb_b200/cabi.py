@@ -343,6 +343,7 @@ _ALGO_SIGS = {
 _PLAN_SIGS = {
     "AggStateCreate": [AggSpec, _VP, C.c_int],
     "ExecuteBatchPlan": [_VP, C.POINTER(BatchPlan), _VP, C.c_int],
+    "ExecuteBatchPlanMulti": [C.POINTER(C.c_void_p), C.c_int, C.POINTER(BatchPlan), _VP, C.c_int],
     "AggStateMerge": [_VP, DimensionVector, _VP, C.c_int, _VP, C.c_int],
     "AggStateGroupCount": [_VP, _VP, C.c_int],
     "AggStateFinalize": [_VP, DimensionVector, _VP, _VP, C.c_int],

@@ -839,8 +839,10 @@ static int classWidth(ValClass c) {
   }
 }
 
-// Translates the ABI plan into the device form, resolving value classes by the reference's rules.
-static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P) {
+// Translates the ABI plan into the device form, resolving value classes by the reference's rules.  `multi` (nmulti
+// states, ExecuteBatchPlanMulti): the plan has one measure root per state, SinkArg = the state's ordinal, each checked
+// against its own state; everything else is taken from `st` (= multi[0]) and the per-measure fields are left to the caller.
+static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P, AggState *const *multi = nullptr, int nmulti = 0) {
   memset(&P, 0, sizeof(P));
   if (bp.NumColumns < 0 || bp.NumColumns > kMaxPlanCols)
     throw EngineError("the fused path stages at most 16 distinct columns per batch");
@@ -884,6 +886,7 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P) {
   std::vector<uint8_t> stack;
   std::vector<bool> dimSeen(RL.numDims, false);
   bool measureSeen = false;
+  std::vector<bool> stateFed(nmulti, false);
   P.lastFilter = -1;
   for (int i = 0; i < bp.NumInsts; i++) {
     const PlanInst &pi = bp.Insts[i];
@@ -958,10 +961,20 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P) {
         break;
       }
       case PLAN_SINK_MEASURE: {
-        if (measureSeen) throw EngineError("only one measure per plan");
+        const AggState *fed = st;
+        if (multi) {
+          if (pi.SinkArg >= nmulti)
+            throw EngineError("measure root with SinkArg " + std::to_string(pi.SinkArg) + ": there are " + std::to_string(nmulti) + " states");
+          if (stateFed[pi.SinkArg]) throw EngineError("two measure roots feed state " + std::to_string(pi.SinkArg) + " (duplicate SinkArg)");
+          stateFed[pi.SinkArg] = true;
+          fed = multi[pi.SinkArg];
+          P.meas[pi.SinkArg].inst = (int8_t)i;
+        } else if (measureSeen) {
+          throw EngineError("only one measure per plan");
+        }
         measureSeen = true;
         ValClass oc = sinkClassOf(pi.SinkDataType, false);
-        if (oc != st->measClass) throw EngineError("measure data type differs from AggSpec.MeasureDataType");
+        if (oc != fed->measClass) throw EngineError("measure data type differs from AggSpec.MeasureDataType");
         I.oclass = oc;
         break;
       }
@@ -972,6 +985,8 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P) {
   for (int d = 0; d < RL.numDims; d++)
     if (!dimSeen[d]) throw EngineError("plan does not produce every dimension of AggSpec");
   if (!measureSeen) throw EngineError("plan has no measure instruction");
+  for (int k = 0; k < nmulti; k++)
+    if (!stateFed[k]) throw EngineError("no measure root feeds state " + std::to_string(k) + " (missing SinkArg)");
   P.hasMeasure = 1;
   P.keyMode = st->keyMode;
   P.rowBytes = (uint8_t)RL.rowBytes;
@@ -1101,17 +1116,22 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
     // not on the batch's ranges.
     for (uint32_t tr : {3968u, 1920u, 896u}) {
       for (uint32_t n = kMaxStages; n >= 2 && !tileRows; n--) {
-        const size_t need = 128 + n * stageBytesFor(tr);
+        // (several measures: one 128-byte aligned region of accumulators each)
+        const size_t need = 128 + n * stageBytesFor(tr) + (P.nmeas > 1 ? 128 * P.nmeas : 0);
         if (need >= (size_t)kSmemBudget) continue;
         // three 32-bit piece counters, or flag + 8-byte accumulator; HLL: one 32-bit map entry (slot -> group's registers)
-        const size_t slotBytes = P.hll ? 4 : P.denseFx ? 12 : 9;
+        size_t slotBytes = P.hll ? 4 : P.denseFx ? 12 : 9;
+        if (P.nmeas > 1) {
+          slotBytes = 0;
+          for (int m = 0; m < P.nmeas; m++) slotBytes += P.meas[m].denseFx ? 12 : 9;
+        }
         uint32_t cap = (uint32_t)(((size_t)kSmemBudget - need) / slotBytes / 16 * 16);
         if (cap > kDenseMaxSlots) cap = kDenseMaxSlots;
         if (cap >= P.denseTotal) { tileRows = tr; stages = n; slots = cap; }
       }
       if (tileRows) break;
     }
-    if (!tileRows && !P.hll && P.neutralSafe && P.denseTotal <= kGlobalDenseMaxSlots) {
+    if (!tileRows && !P.hll && P.nmeas <= 1 && P.neutralSafe && P.denseTotal <= kGlobalDenseMaxSlots) {
       // more slots than a CTA holds: one accumulator array in global memory for the whole grid; shared memory is all ring
       for (uint32_t tr : {3968u, 1920u, 896u}) {
         const uint32_t n = stagesIn((size_t)kSmemBudget - 128 - 256, tr);
@@ -1130,6 +1150,7 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
     if (tileRows && fullTiles(tileRows) == 0) { tileRows = 0; slots = 8192; }
     if (!tileRows) { P.denseNd = 0; P.denseGlobal = 0; }
   }
+  if (!tileRows && P.nmeas > 1) { P.denseNd = 0; return 0; }   // several measures share only the CTA's direct-indexed slots
   if (!tileRows) {
     for (uint32_t sl : {slots, slots / 2, slots / 4}) {
       for (uint32_t tr : {3968u, 1920u, 896u}) {  // 128 rows x (31 | 15 | 7) consumer warps
@@ -1171,6 +1192,10 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
   P.stageBytes = (uint32_t)stageBytes;
   P.smemSlots = slots;
   P.tableBytes = P.denseNd != 0 ? (slots * (P.hll ? 4 : P.denseFx ? 12 : 9) + 127) / 128 * 128 : slots * 8;
+  if (P.nmeas > 1) {
+    P.tableBytes = 0;
+    for (int m = 0; m < P.nmeas; m++) P.tableBytes += (slots * (P.meas[m].denseFx ? 12 : 9) + 127) / 128 * 128;
+  }
   return 128 + (size_t)P.tableBytes + stageBytes * P.numStages;
 }
 
@@ -1366,16 +1391,8 @@ static void prepareInputs(DevPlan &P, const BatchPlan &bp, cudaStream_t s, std::
   }
 }
 
-static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
-  if (bp.NumRows == 0) return;
-  if (bp.NumRows > 0x7FFFFFFFu) throw EngineError("a batch holds at most 2^31-1 rows");
-  static thread_local DevPlan P;  // ~3 KB
-  compilePlan(st, bp, P);
-  P.resume = 0;
-  std::vector<std::unique_ptr<Scratch>> scratch;   // expanded / realigned columns, run hints: released in stream order
-  prepareInputs(P, bp, s, &scratch);
-  // joined dimension tables: indexes + foreign-column batches go to device memory for the kernel's lifetime
-  std::unique_ptr<Scratch> joinMem;
+// Joined dimension tables: indexes + foreign-column batches go to device memory for the kernel's lifetime (joinMem).
+static void uploadJoin(DevPlan &P, const BatchPlan &bp, cudaStream_t s, std::unique_ptr<Scratch> &joinMem) {
   P.join = nullptr;
   if (P.numForeignCols > 0 || P.numForeignTables > 0) {
     static thread_local DevJoin J;
@@ -1394,8 +1411,10 @@ static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
     ARES_CUDA(cudaStreamSynchronize(s));   // J is reused by the next call of this thread
     P.join = joinMem->as<DevJoin>();
   }
-  size_t smemBytes = layoutStages(P, st->spec.ExpectedGroups);
-  // per-tile run hints of the first-class RLE columns (the tile size is known now)
+}
+
+// Per-tile run hints of the first-class RLE columns (after layoutStages: the tile size is known).
+static void rleTileHints(DevPlan &P, const BatchPlan &bp, cudaStream_t s, std::vector<std::unique_ptr<Scratch>> &scratch) {
   for (int c = 0; c < P.ncols; c++) {
     DevColumn &col = P.cols[c];
     if (!col.rle) continue;
@@ -1406,15 +1425,34 @@ static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
     checkLastError("rleTileRuns");
     col.tileRun = scratch.back()->as<uint32_t>();
   }
+}
+
+// one CTA per SM, or per full tile when there are fewer; a batch without a full tile is the tail of one CTA
+static int launchGrid(const DevPlan &P) {
+  int grid = smCount() < kMaxGridCtas ? smCount() : kMaxGridCtas;
+  if ((uint32_t)grid > P.numFullTiles) grid = P.numFullTiles ? (int)P.numFullTiles : 1;
+  return grid;
+}
+
+static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
+  if (bp.NumRows == 0) return;
+  if (bp.NumRows > 0x7FFFFFFFu) throw EngineError("a batch holds at most 2^31-1 rows");
+  static thread_local DevPlan P;  // ~3 KB
+  compilePlan(st, bp, P);
+  P.resume = 0;
+  std::vector<std::unique_ptr<Scratch>> scratch;   // expanded / realigned columns, run hints: released in stream order
+  prepareInputs(P, bp, s, &scratch);
+  std::unique_ptr<Scratch> joinMem;
+  uploadJoin(P, bp, s, joinMem);
+  size_t smemBytes = layoutStages(P, st->spec.ExpectedGroups);
+  rleTileHints(P, bp, s, scratch);
   // room in the group table (see "growth of the group table"): the direct-indexed kernels are not waited for, so what
   // they may insert is reserved up front (flush of the CTA slots / fold of the global slot array; out-of-range rows
   // park); hash-table kernels are checked after the launch and resumed when they stopped.
   const bool resumable = P.denseNd == 0 && !st->hllDense;
   if (!resumable && !st->hllDense) ensureRoom(st, (uint64_t)P.denseTotal, s);
   P.ctaAcc = st->ctaAcc;   // (after a possible growth: the slices live in the table's allocation)
-  // one CTA per SM, or per full tile when there are fewer; a batch without a full tile is the tail of one CTA
-  int grid = smCount() < kMaxGridCtas ? smCount() : kMaxGridCtas;
-  if ((uint32_t)grid > P.numFullTiles) grid = P.numFullTiles ? (int)P.numFullTiles : 1;
+  const int grid = launchGrid(P);
   if (P.denseGlobal) {
     if (!st->denseAcc) {   // first use: 16 MB of accumulators at the neutral element (denseFoldKernel leaves them so)
       st->denseAcc = static_cast<unsigned long long *>(deviceAllocOrThrow((size_t)kGlobalDenseMaxSlots * sizeof(unsigned long long)));
@@ -1466,6 +1504,121 @@ static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
     P.resume = 1;
     P.ctaAcc = st->ctaAcc;
   }
+}
+
+// ---------------------------------------------------------------------------------------
+// several measures over one scan (ExecuteBatchPlanMulti)
+// ---------------------------------------------------------------------------------------
+// States that may share a plan: the same dimension layout and reduce mode, no HLL.
+static void checkSharedStates(AggState *const *sts, int n) {
+  if (n < 1 || n > kJitMaxMeasures) throw EngineError("numStates must be 1.." + std::to_string(kJitMaxMeasures));
+  for (int k = 0; k < n; k++) {
+    if (sts[k]->hll) throw EngineError("AGGR_HLL states cannot share a plan");
+    if (memcmp(sts[k]->spec.NumDimsPerDimWidth, sts[0]->spec.NumDimsPerDimWidth, NUM_DIM_WIDTH) != 0)
+      throw EngineError("states differ in NumDimsPerDimWidth");
+    if (sts[k]->spec.ReduceMode != sts[0]->spec.ReduceMode) throw EngineError("states differ in ReduceMode");
+  }
+}
+
+// Single-measure plans of the states of a shared plan (BatchPlan has no default constructor: raw storage).
+struct MeasurePlans {
+  std::vector<unsigned char> mem;
+  void resize(int n) { mem.resize(sizeof(BatchPlan) * n); }
+  BatchPlan &operator[](int k) { return reinterpret_cast<BatchPlan *>(mem.data())[k]; }
+};
+
+// The single-measure plan of state k: every instruction except the other states' measure roots and the sub-expressions
+// only they consume.
+static void measurePlan(const BatchPlan &bp, int k, BatchPlan &out) {
+  std::vector<std::vector<int>> stack;   // instructions of each stacked sub-expression
+  std::vector<bool> drop(bp.NumInsts, false);
+  for (int i = 0; i < bp.NumInsts; i++) {
+    const PlanInst &pi = bp.Insts[i];
+    std::vector<int> tree{i};
+    auto pop = [&] {
+      if (stack.empty()) throw EngineError("plan pops an empty evaluation stack");
+      tree.insert(tree.end(), stack.back().begin(), stack.back().end());
+      stack.pop_back();
+    };
+    if (pi.NumOperands == 2 && pi.B.Kind == PLAN_OPERAND_STACK) pop();
+    if (pi.A.Kind == PLAN_OPERAND_STACK) pop();
+    if (pi.Sink == PLAN_SINK_STACK) stack.push_back(tree);
+    if (pi.Sink == PLAN_SINK_MEASURE && pi.SinkArg != k)
+      for (int j : tree) drop[j] = true;
+  }
+  memcpy(&out, &bp, sizeof(BatchPlan));
+  int n = 0;
+  for (int i = 0; i < bp.NumInsts; i++) {
+    if (drop[i]) continue;
+    out.Insts[n] = bp.Insts[i];
+    if (out.Insts[n].Sink == PLAN_SINK_MEASURE) out.Insts[n].SinkArg = 0;
+    n++;
+  }
+  out.NumInsts = n;
+}
+
+// Compiles the shared plan into P and decides its form for this batch.  true: one kernel feeds every state — each
+// measure's own single-measure plan takes the CTA's direct-indexed slots, and all of them fit a CTA together (P is then
+// laid out, without device work when `scratch` is null).  false: the caller runs subs[k] on state k, one kernel each.
+// `subs` is filled either way.
+static bool planShared(AggState *const *sts, int n, const BatchPlan &bp, DevPlan &P, MeasurePlans &subs,
+                       cudaStream_t s, std::vector<std::unique_ptr<Scratch>> *scratch) {
+  compilePlan(sts[0], bp, P, sts, n);
+  subs.resize(n);
+  for (int k = 0; k < n; k++) measurePlan(bp, k, subs[k]);
+  if (bp.NumRows == 0) return false;
+  static thread_local DevPlan Q;
+  bool shared = true;
+  bool skipCount = true;
+  for (int k = 0; k < n; k++) {
+    compilePlan(sts[k], subs[k], Q);
+    prepareInputs(Q, subs[k], nullptr, nullptr);
+    layoutStages(Q, sts[k]->spec.ExpectedGroups);
+    shared = shared && Q.denseNd != 0 && !Q.denseGlobal;
+    DevMeasure &M = P.meas[k];
+    M.aggOp = Q.aggOp; M.measWidth = Q.measWidth; M.skipCount = Q.skipCount; M.neutralSafe = Q.neutralSafe;
+    M.denseFx = Q.denseFx; M.fxShift = Q.fxShift; M.measureIdentity = Q.measureIdentity; M.accNeutral = Q.accNeutral;
+    skipCount = skipCount && Q.skipCount;
+  }
+  if (!shared) return false;
+  P.nmeas = (uint8_t)n;
+  P.skipCount = skipCount;   // base counts are staged when some measure counts run lengths
+  static thread_local DevPlan D;
+  D = P;   // the layout decision first, on a copy: prepareInputs rewrites the column descriptors
+  prepareInputs(D, bp, s, nullptr);
+  uint32_t expected = 0;
+  for (int k = 0; k < n; k++) expected = sts[k]->spec.ExpectedGroups > expected ? sts[k]->spec.ExpectedGroups : expected;
+  if (layoutStages(D, expected) == 0) return false;
+  if (scratch == nullptr) { P = D; return true; }
+  prepareInputs(P, bp, s, scratch);
+  layoutStages(P, expected);
+  return P.denseNd != 0;
+}
+
+static void executePlanMulti(AggState *const *sts, int n, const BatchPlan &bp, cudaStream_t s) {
+  checkSharedStates(sts, n);
+  if (n == 1) { executePlan(sts[0], bp, s); return; }
+  if (bp.NumRows > 0x7FFFFFFFu) throw EngineError("a batch holds at most 2^31-1 rows");
+  static thread_local DevPlan P;
+  MeasurePlans subs;
+  std::vector<std::unique_ptr<Scratch>> scratch;
+  if (!planShared(sts, n, bp, P, subs, s, &scratch)) {
+    for (int k = 0; k < n; k++) executePlan(sts[k], subs[k], s);
+    return;
+  }
+  P.resume = 0;
+  std::unique_ptr<Scratch> joinMem;
+  uploadJoin(P, bp, s, joinMem);
+  const size_t smemBytes = 128 + (size_t)P.tableBytes + (size_t)P.stageBytes * P.numStages;
+  rleTileHints(P, bp, s, scratch);
+  // direct-indexed kernels are not waited for: every state gets room for what the flush may insert up front
+  for (int k = 0; k < n; k++) {
+    ensureRoom(sts[k], (uint64_t)P.denseTotal, s);
+    P.meas[k].G = sts[k]->table;
+    P.meas[k].ctaAcc = sts[k]->ctaAcc;
+  }
+  P.ctaAcc = sts[0]->ctaAcc;
+  jitLaunch(P, sts[0]->table, smemBytes, launchGrid(P), s);
 }
 
 static void mergeRows(AggState *st, const DimensionVector &in, const uint8_t *values, int length, cudaStream_t s) {
@@ -1801,6 +1954,17 @@ CGoCallResHandle ExecuteBatchPlan(void *state, const BatchPlan *plan, void *cuda
   });
 }
 
+CGoCallResHandle ExecuteBatchPlanMulti(void *const *states, int numStates, const BatchPlan *plan, void *cudaStream, int device) {
+  return guarded("ExecuteBatchPlanMulti", device, [&]() -> int64_t {
+    if (!plan) throw EngineError("null plan");
+    if (!states || numStates < 1 || numStates > kJitMaxMeasures) throw EngineError("numStates must be 1.." + std::to_string(kJitMaxMeasures));
+    AggState *sts[kJitMaxMeasures];
+    for (int k = 0; k < numStates; k++) sts[k] = asState(states[k]);
+    executePlanMulti(sts, numStates, *plan, (cudaStream_t)cudaStream);
+    return 0;
+  });
+}
+
 CGoCallResHandle AggStateMerge(void *state, DimensionVector inputKeys, uint8_t *inputValues, int length,
                                void *cudaStream, int device) {
   return guarded("AggStateMerge", device, [&]() -> int64_t {
@@ -1945,6 +2109,41 @@ CGoCallResHandle AresJitDryRun(AggSpec spec, const BatchPlan *plan, char **sourc
     h.res = reinterpret_cast<void *>(n);
   } catch (const std::exception &e) {
     h.pStrErr = strdup((std::string("AresJitDryRun: ") + e.what()).c_str());
+  }
+  return h;
+}
+
+// Additive diagnostics, usable without a GPU: the kernel of a plan whose measure roots feed numSpecs states (the shared
+// form of ExecuteBatchPlanMulti for this batch's zone map), generated and compiled; res = cubin size.  A plan that would
+// run as one kernel per state (no shared form for this batch) is reported as an error.
+CGoCallResHandle AresJitDryRunMulti(const AggSpec *specs, int numSpecs, const BatchPlan *plan, char **sourceOut) {
+  CGoCallResHandle h = {nullptr, nullptr};
+  try {
+    if (!specs || !plan || numSpecs < 1 || numSpecs > kJitMaxMeasures) throw EngineError("numSpecs must be 1.." + std::to_string(kJitMaxMeasures));
+    std::vector<AggState> st(numSpecs);
+    AggState *sts[kJitMaxMeasures];
+    for (int k = 0; k < numSpecs; k++) {
+      memset(&st[k].table, 0, sizeof(st[k].table));
+      describeState(&st[k], specs[k]);
+      st[k].capacity = 0;
+      sts[k] = &st[k];
+    }
+    checkSharedStates(sts, numSpecs);
+    static thread_local DevPlan P;
+    MeasurePlans subs;
+    if (numSpecs == 1) {
+      compilePlan(sts[0], *plan, P);
+      prepareInputs(P, *plan, nullptr, nullptr);
+      layoutStages(P, specs[0].ExpectedGroups);
+    } else if (!planShared(sts, numSpecs, *plan, P, subs, nullptr, nullptr)) {
+      throw EngineError("this plan and zone map run one kernel per state (no shared direct-indexed form)");
+    }
+    std::string src;
+    size_t n = jitCompileOnly(P, &src);
+    if (sourceOut) *sourceOut = strdup(src.c_str());
+    h.res = reinterpret_cast<void *>(n);
+  } catch (const std::exception &e) {
+    h.pStrErr = strdup((std::string("AresJitDryRunMulti: ") + e.what()).c_str());
   }
   return h;
 }

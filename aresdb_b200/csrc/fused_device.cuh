@@ -91,6 +91,9 @@ __device__ __forceinline__ uint32_t globalHome(const DevTable &G, unsigned long 
 }
 
 // spillWhenStopped: a NEW key is not claimed once the stop flag is up (kSlotSpill: the caller parks the row).
+// `Table`: a kernel that feeds several group tables calls one instantiation per table — lanes claiming in different tables
+// then run different code, so the warp-aggregated claim counter below only ever combines lanes of one table.
+template <int Table = 0>
 static __device__ __noinline__ uint32_t globalFindOrClaim(const DevTable &G, unsigned long long key, const uint64_t *roww,
                                                           bool spillWhenStopped = false) {
   uint32_t slot = globalHome(G, key);
@@ -141,9 +144,10 @@ static __device__ __noinline__ void globalPark(const DevTable &G, unsigned long 
   }
 }
 
+template <int Table = 0>
 __device__ __forceinline__ void globalUpdate(const DevTable &G, AggOp op, unsigned long long key, const uint64_t *roww,
                                              uint64_t val, bool spillWhenStopped = false) {
-  uint32_t slot = globalFindOrClaim(G, key, roww, spillWhenStopped);
+  uint32_t slot = globalFindOrClaim<Table>(G, key, roww, spillWhenStopped);
   if (slot == kSlotSpill) { globalPark(G, key, roww, val); return; }
   if (slot != 0xFFFFFFFFu) aggAtomic(op, &G.acc[slot], val);
 }

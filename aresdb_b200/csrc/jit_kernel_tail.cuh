@@ -3,7 +3,10 @@
 // CTA-private shared table, and the flush into the global table.  The shape macros
 // (JIT_TILE_ROWS, JIT_STAGE_BYTES, JIT_SMEM_SLOTS, JIT_KW, JIT_AGG_OP, JIT_HASH_BITS,
 // JIT_ROW_BYTES, JIT_THREADS, JIT_NUM_PARTS + kPartSmemOff/kPartBytes/kPartTileStride) and
-// rowEval() precede this text.
+// rowEval() precede this text.  JIT_NMEAS > 1: the plan's measure roots feed that many states (direct-indexed form).
+#ifndef JIT_NMEAS
+#define JIT_NMEAS 1
+#endif
 namespace aresb {
 
 __device__ __forceinline__ void jitIssueTile(const JitParams &P, uint32_t tile, uint8_t *stage, uint64_t *bar) {
@@ -35,6 +38,7 @@ __device__ __forceinline__ unsigned long long jitKeyOf(const uint64_t (&key)[4][
 //   * rows inside whose value would leave a flag-less slot at its neutral element: the hash table as well;
 //   * integer form: rows inside whose value is off the 2^-S grid: added in double on the CTA's L2 slice at `slot`
 //     (-0.0, which would leave that half at its neutral element: the hash table).
+#if JIT_NMEAS == 1
 static __device__ __noinline__ void denseColdRows(const uint8_t *stage, uint32_t q, uint32_t row0, const JitParams &P, uint32_t nvalid,
                                                   uint32_t inRange, uint32_t s0, uint32_t s1, uint32_t s2, uint32_t s3,
                                                   unsigned long long *tAcc) {
@@ -63,6 +67,7 @@ static __device__ __noinline__ void denseColdRows(const uint8_t *stage, uint32_t
     if (toHash) globalUpdate(P.G, (AggOp)JIT_AGG_OP, jitKeyOfRow(key[r]), JIT_KW == 1 ? nullptr : key[r], meas[r], /*spillWhenStopped=*/true);
   }
 }
+#endif
 
 // Where the accumulators of the direct-indexed slots live (JIT_DENSE_ACC, chosen by the host):
 //   1  shared memory (native ATOMS): 4-byte aggregates other than float min / max;
@@ -147,6 +152,7 @@ static __device__ __noinline__ void denseColdRowsHll(const uint8_t *stage, uint3
 }
 
 // `repOff`: this lane's copy of the slots (few slots are replicated per lane), in slots — loop invariant, computed once.
+#if JIT_NMEAS == 1
 __device__ __forceinline__ void jitAggregateDense(uint32_t touchedAddr, unsigned long long *tAcc, const JitParams &P, const uint8_t *stage,
                                                   uint32_t q, uint32_t row0, uint32_t nvalid, uint32_t repOff, const bool (&fast)[4],
                                                   bool cold, const uint32_t (&dslot)[4], const uint64_t (&meas)[4],
@@ -251,6 +257,179 @@ __device__ __forceinline__ void jitAggregateDense(uint32_t touchedAddr, unsigned
 }
 #endif
 
+#if JIT_NMEAS > 1
+// ---- several measures, one pass (ExecuteBatchPlanMulti) ---------------------------------------------------------------
+// A row is evaluated once (filters, dimensions, slot); measure M's value goes to its own accumulators: region
+// kMeasSmemOff[M] of the table area (three 12-byte piece counters per slot, or a flag byte per slot followed by 8-byte
+// accumulators), the CTA's slice of its state's ctaAcc, and — for rows the fast path cannot finish — its state's group
+// table.  Each measure keeps the form its single-measure plan takes (kMeasAcc / kMeasFlags / kMeasCheck are JIT_DENSE_ACC
+// / JIT_DENSE_FLAGS / JIT_DENSE_CHECK of that plan), with the same rules as jitAggregateDense / denseColdRows.
+// STEP(M) for every measure M (indexes past JIT_NMEAS fold to 0 in code that never runs)
+#define JIT_EACH_MEASURE(STEP) { STEP(0) STEP(1) if (JIT_NMEAS > 2) { STEP((JIT_NMEAS > 2 ? 2 : 0)) } if (JIT_NMEAS > 3) { STEP((JIT_NMEAS > 3 ? 3 : 0)) } }
+template <int M>
+__device__ __forceinline__ unsigned long long *measSlice(const JitParams &P) { return P.ms[M].ctaAcc + (size_t)blockIdx.x * JIT_SMEM_SLOTS; }
+
+template <int M>
+__device__ __forceinline__ void multiColdMeasure(const JitParams &P, uint32_t alive, uint32_t inRange, const uint64_t (&key)[4][JIT_KW],
+                                                 const uint64_t (&meas)[4], const uint32_t (&slot)[4]) {
+  constexpr int OP = kMeasOp[M];
+  unsigned long long *tAcc = measSlice<M>(P);
+#pragma unroll
+  for (int r = 0; r < 4; r++) {
+    if (!((alive >> r) & 1u)) continue;
+    if ((inRange >> r) & 1u) {
+      if (kMeasAcc[M] == 4) {
+        const float x = (float)__longlong_as_double((long long)meas[r]);
+        const float y = x * P.ms[M].fxScale;
+        const bool onGrid = x > 0.0f && y < 4294967296.0f && __uint2float_rn(__float2uint_rz(y)) == y;
+        if (onGrid) continue;
+        if (meas[r] != 0x8000000000000000ull) { aggAtomic((AggOp)OP, tAcc + slot[r], meas[r]); continue; }
+      } else {
+        if (kMeasFlags[M] || !kMeasCheck[M] || meas[r] != P.ms[M].accNeutral) continue;
+      }
+    }
+    globalUpdate<M>(P.ms[M].G, (AggOp)OP, jitKeyOfRow(key[r]), JIT_KW == 1 ? nullptr : key[r], meas[r], /*spillWhenStopped=*/true);
+  }
+}
+
+// the rows some measure's fast path could not finish, evaluated again with full generality (out of line, rare)
+static __device__ __noinline__ void multiColdRows(const uint8_t *stage, uint32_t q, uint32_t row0, const JitParams &P, uint32_t nvalid,
+                                                  uint32_t inRange, uint32_t s0, uint32_t s1, uint32_t s2, uint32_t s3) {
+  uint64_t key[4][JIT_KW], mv[JIT_NMEAS][4];
+  const uint32_t slot[4] = {s0, s1, s2, s3};
+  uint32_t alive = rowEvalGeneric(stage, q, row0, P, key, mv[0] JIT_MEAS_REST1(mv));
+  alive &= (1u << nvalid) - 1u;
+#define JIT_STEP(M) multiColdMeasure<M>(P, alive, inRange, key, mv[M], slot);
+  JIT_EACH_MEASURE(JIT_STEP)
+#undef JIT_STEP
+}
+
+template <int M>
+__device__ __forceinline__ bool multiDenseMeasure(uint32_t tableAddr, const JitParams &P, const bool (&fast)[4], const uint32_t (&s)[4],
+                                                  const uint64_t (&meas)[4], const uint32_t (&mraw)[4]) {
+  constexpr int OP = kMeasOp[M];
+  const uint32_t base = tableAddr + kMeasSmemOff[M];
+  bool cold = false;
+  if (kMeasAcc[M] == 4) {
+#pragma unroll
+    for (int r = 0; r < 4; r++) {
+      const float x = __uint_as_float(mraw[r]);
+      const float y = x * P.ms[M].fxScale;
+      const uint32_t ix = __float2uint_rz(y);
+      const bool onGrid = fast[r] && x > 0.0f && y < 4294967296.0f && __uint2float_rn(ix) == y;
+      cold = cold || (fast[r] && !onGrid);
+      if (onGrid) {
+        const uint32_t a = base + 12u * s[r];
+        asm volatile("red.shared.add.u32 [%0], %1;\n\tred.shared.add.u32 [%0+4], %2;\n\tred.shared.add.u32 [%0+8], %3;"
+                     ::"r"(a), "r"(ix & 0x7FFu), "r"((ix >> 11) & 0x7FFu), "r"(ix >> 22) : "memory");
+      }
+    }
+  } else {
+    bool go[4];
+#pragma unroll
+    for (int r = 0; r < 4; r++) {
+      go[r] = fast[r] && (kMeasFlags[M] || !kMeasCheck[M] || meas[r] != P.ms[M].accNeutral);
+      cold = cold || (fast[r] && !go[r]);
+    }
+    if (kMeasFlags[M]) {
+#pragma unroll
+      for (int r = 0; r < 4; r++) stsFlag(base + s[r], go[r]);
+    }
+    unsigned long long *tAcc = measSlice<M>(P);
+    unsigned long long *generic = reinterpret_cast<unsigned long long *>(denseSmemBase() + kMeasSmemOff[M] + kDenseCap);
+    constexpr int kToShared = kMeasAcc[M] == 1 ? 4 : 2;
+#pragma unroll
+    for (int r = 0; r < 4; r++) {
+      if (r < kToShared) redSharedPred<OP>(base + kDenseCap + 8u * s[r], generic + s[r], meas[r], go[r]);
+      else redGlobalPred<OP>(tAcc + s[r], meas[r], go[r]);
+    }
+  }
+  return cold;
+}
+
+__device__ __forceinline__ void multiAggregateDense(uint32_t tableAddr, const JitParams &P, const uint8_t *stage, uint32_t q, uint32_t row0,
+                                                    uint32_t nvalid, uint32_t repOff, const bool (&fast)[4], bool cold,
+                                                    const uint32_t (&dslot)[4], const uint64_t (&mv)[JIT_NMEAS][4],
+                                                    const uint32_t (&mr)[JIT_NMEAS][4]) {
+  uint32_t s[4];
+#pragma unroll
+  for (int r = 0; r < 4; r++) s[r] = dslot[r] + repOff;
+#define JIT_STEP(M) cold = multiDenseMeasure<M>(tableAddr, P, fast, s, mv[M], mr[M]) || cold;
+  JIT_EACH_MEASURE(JIT_STEP)
+#undef JIT_STEP
+  if (cold) {
+    const uint32_t inRange = (fast[0] ? 1u : 0u) | (fast[1] ? 2u : 0u) | (fast[2] ? 4u : 0u) | (fast[3] ? 8u : 0u);
+    multiColdRows(stage, q, row0, P, nvalid, inRange, s[0], s[1], s[2], s[3]);
+  }
+}
+
+template <int M>
+__device__ __forceinline__ void multiInitMeasure(const JitParams &P, uint32_t denseSlots) {
+  {
+    uint8_t *base = denseSmemBase() + kMeasSmemOff[M];
+    unsigned long long *tAcc = measSlice<M>(P);
+    for (uint32_t i = threadIdx.x; i < denseSlots; i += JIT_THREADS) {
+      if (kMeasAcc[M] != 1) tAcc[i] = P.ms[M].accNeutral;
+      if (kMeasAcc[M] == 4) {
+        uint32_t *c = reinterpret_cast<uint32_t *>(base) + 3u * i;
+        c[0] = 0; c[1] = 0; c[2] = 0;
+      } else {
+        if (kMeasFlags[M]) base[i] = 0;
+        reinterpret_cast<unsigned long long *>(base + kDenseCap)[i] = P.ms[M].accNeutral;
+      }
+    }
+  }
+}
+__device__ __forceinline__ void multiInit(const JitParams &P, uint32_t denseSlots) {
+#define JIT_STEP(M) multiInitMeasure<M>(P, denseSlots);
+  JIT_EACH_MEASURE(JIT_STEP)
+#undef JIT_STEP
+}
+
+// the CTA's slots of every measure into its state's group table (as the single-measure flush)
+template <int M>
+__device__ __forceinline__ void multiFlushMeasure(const JitParams &P, uint32_t denseSlots) {
+  {
+    constexpr int OP = kMeasOp[M];
+    const uint8_t *base = denseSmemBase() + kMeasSmemOff[M];
+    unsigned long long *tAcc = measSlice<M>(P);
+    const unsigned long long neutral = P.ms[M].accNeutral;
+    for (uint32_t i = threadIdx.x; i < denseSlots; i += JIT_THREADS) {
+      unsigned long long accS = neutral;
+      if (kMeasAcc[M] == 4) {
+        const uint32_t *c = reinterpret_cast<const uint32_t *>(base) + 3u * i;
+        const unsigned long long v = (unsigned long long)c[0] + ((unsigned long long)c[1] << 11) + ((unsigned long long)c[2] << 22);
+        if (v != 0) accS = (unsigned long long)__double_as_longlong(__ull2double_rn(v) * P.ms[M].fxInv);
+      } else {
+        accS = reinterpret_cast<const unsigned long long *>(base + kDenseCap)[i];
+      }
+      const unsigned long long accG = kMeasAcc[M] != 1 ? __ldcg(&tAcc[i]) : neutral;
+      if (kMeasFlags[M] ? !base[i] : (accS == neutral && accG == neutral)) continue;
+      uint32_t rem = i % P.dRepStride, dvr[JIT_ND], vb = 0;
+#pragma unroll
+      for (int k = JIT_ND - 1; k >= 0; k--) {
+        const uint32_t ix = rem / P.dStride[k];
+        rem -= ix * P.dStride[k];
+        const bool valid = ix != P.dCnt[k];
+        dvr[k] = valid ? (P.dLo[k] + ix) * P.dStep[k] : 0u;
+        vb |= (valid ? 1u : 0u) << k;
+      }
+      uint64_t key[JIT_KW];
+      densePack(dvr, vb, key);
+      const unsigned long long k = jitKeyOfRow(key);
+      if (kMeasAcc[M] != 1) globalUpdate<M>(P.ms[M].G, (AggOp)OP, k, JIT_KW == 1 ? nullptr : key, accG, true);
+      globalUpdate<M>(P.ms[M].G, (AggOp)OP, k, JIT_KW == 1 ? nullptr : key, accS, true);
+    }
+  }
+}
+__device__ __forceinline__ void multiFlush(const JitParams &P, uint32_t denseSlots) {
+#define JIT_STEP(M) multiFlushMeasure<M>(P, denseSlots);
+  JIT_EACH_MEASURE(JIT_STEP)
+#undef JIT_STEP
+}
+#endif
+#endif
+
 // Folds the surviving rows of one quad.  Normal mode: the CTA's shared table first, the global table
 // for rows it cannot take (counted in *misses).  Bypass mode (the batch has far more groups than the
 // shared table holds, so looking there is wasted work): straight to the L2-resident global table,
@@ -330,8 +509,11 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
   asm volatile("" : "+r"(touchedAddr));   // keep it in a register: the compiler otherwise rebuilds the window address per store
   const uint32_t denseSlots = JIT_DENSE == 2 ? 0u : P.dRepStride * P.dReps;   // <= kDenseCap (host); 2: nothing CTA-private
   const uint32_t repOff = JIT_DENSE == 2 ? (blockIdx.x & (P.dReps - 1u)) * P.dRepStride : (threadIdx.x & (P.dReps - 1u)) * P.dRepStride *
-                                                (JIT_DENSE_ACC == 4 ? 12u : 1u);   // this lane's copy of the slots (integer form: in bytes)
+                                                (JIT_DENSE_ACC == 4 && JIT_NMEAS == 1 ? 12u : 1u);   // this lane's copy of the slots (integer form: in bytes)
   for (uint32_t i = threadIdx.x; JIT_HLL == 2 && i < denseSlots; i += JIT_THREADS) reinterpret_cast<uint32_t *>(tKeys)[i] = 0xFFFFFFFFu;
+#if JIT_NMEAS > 1
+  multiInit(P, denseSlots);
+#else
   for (uint32_t i = threadIdx.x; JIT_HLL != 2 && i < denseSlots; i += JIT_THREADS) {
     if (JIT_DENSE_FLAGS) touched[i] = 0;
     if (JIT_DENSE_ACC != 1) tAcc[i] = P.accNeutral;
@@ -342,6 +524,7 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
       denseSharedAcc()[i] = P.accNeutral;
     }
   }
+#endif
 #else
   for (uint32_t i = threadIdx.x; i < JIT_SMEM_SLOTS; i += JIT_THREADS) {
     tKeys[i] = kEmptyKey;
@@ -411,7 +594,15 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
       {
         const uint32_t q = threadIdx.x;
         uint64_t meas[4];
-#if JIT_DENSE
+#if JIT_DENSE && JIT_NMEAS > 1
+        uint32_t dslot[4];
+        bool fast[4], anySlow;
+        uint64_t mv[JIT_NMEAS][4];
+        uint32_t mr[JIT_NMEAS][4];
+        if (rowEval(stage, q, t * JIT_TILE_ROWS + q * 4, P, 4u, fast, anySlow, dslot, mv[0], mr[0] JIT_MEAS_REST(mv, mr)))
+          multiAggregateDense(touchedAddr, P, stage, q, t * JIT_TILE_ROWS + q * 4, 4u, repOff, fast, anySlow, dslot, mv, mr);
+        (void)meas; (void)allowClaim; (void)bypass;
+#elif JIT_DENSE
         uint32_t dslot[4];
         bool fast[4], anySlow;
         uint32_t mraw[4];
@@ -463,7 +654,15 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
       for (uint32_t q = threadIdx.x; q * 4 < rows; q += JIT_THREADS) {
         uint64_t meas[4];
         const uint32_t nvalid = rows - q * 4 < 4 ? rows - q * 4 : 4;
-#if JIT_DENSE
+#if JIT_DENSE && JIT_NMEAS > 1
+        uint32_t dslot[4];
+        bool fast[4], anySlow;
+        uint64_t mv[JIT_NMEAS][4];
+        uint32_t mr[JIT_NMEAS][4];
+        if (rowEval(stages, q, done + q * 4, P, nvalid, fast, anySlow, dslot, mv[0], mr[0] JIT_MEAS_REST(mv, mr)))
+          multiAggregateDense(touchedAddr, P, stages, q, done + q * 4, nvalid, repOff, fast, anySlow, dslot, mv, mr);
+        (void)meas;
+#elif JIT_DENSE
         uint32_t dslot[4];
         bool fast[4], anySlow;
         uint32_t mraw[4];
@@ -483,6 +682,9 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
   if (JIT_HLL == 2) return;  // nothing CTA-private to fold: registers are updated in place
 #if JIT_DENSE == 2
   return;   // denseFoldKernel (batch_plan.cu) folds the shared array after the batch
+#elif JIT_DENSE && JIT_NMEAS > 1
+  multiFlush(P, denseSlots);
+  return;
 #elif JIT_DENSE
   // fold the touched slots into the global table: the slot index decodes to the dimension values
   for (uint32_t i = threadIdx.x; i < denseSlots; i += JIT_THREADS) {

@@ -25,6 +25,7 @@ constexpr int kJitMaxWide = 8;
 constexpr int kJitMaxMagic = 16;
 constexpr int kJitMaxDenseDims = 8;
 constexpr int kJitMaxRle = 4;
+constexpr int kJitMaxMeasures = 4;   // measure roots of one plan, each feeding its own AggState (ExecuteBatchPlanMulti)
 // A mode-3 column read by the kernel straight from its runs: cumulative counts (length + 1 entries), null bitmap and
 // values of the RUNS, and the per-tile run hint computed by rleTileRunsKernel.
 struct RleColumn {
@@ -32,6 +33,17 @@ struct RleColumn {
   const uint8_t *nulls, *values;
   const uint32_t *tileRun;
   uint32_t length, startBit;
+};
+
+// One measure of a plan whose measure roots feed several states (JIT_NMEAS > 1): the state's group table, its CTA slices
+// and the constants the single-measure kernel takes from JitParams' own fields.
+struct JitMeasure {
+  DevTable G;
+  unsigned long long *ctaAcc;
+  unsigned long long measureIdentity, accNeutral;
+  double fxInv;
+  float fxScale;
+  uint32_t pad;
 };
 
 struct JitParams {
@@ -60,7 +72,9 @@ struct JitParams {
   uint32_t resume;                        // 1: second launch of the same batch after the table grew (progress[] says where)
   uint32_t startCount;                    // row number of index position 0 when the batch has no base counts
   RleColumn rle[kJitMaxRle];              // run-length encoded columns decoded in place (see ldrle)
+  JitMeasure ms[kJitMaxMeasures];         // JIT_NMEAS > 1: measure m's state (unused by single-measure kernels)
 };
+// (with every measure's group table in it: the block stays far below the 32 KB kernel-parameter limit of sm_90)
 static_assert(sizeof(JitParams) <= 4096, "the kernel's parameter block is limited to 4 KB");
 
 }  // namespace aresb

@@ -46,6 +46,17 @@ struct DevInst {
   uint8_t rowOff, width, nullOff, pad;
 };
 
+// One measure root of a plan that feeds several states (DevPlan::nmeas > 1): what the single-measure plan of its state
+// decided (compilePlan + layoutStages on that plan), so that each measure takes the accumulation form it would take alone.
+struct DevMeasure {
+  DevTable G;                    // the state's group table and CTA slices (filled just before the launch)
+  unsigned long long *ctaAcc;
+  uint64_t measureIdentity, accNeutral;
+  int8_t inst;                   // the measure root in the shared plan
+  int8_t fxShift;
+  uint8_t aggOp, measWidth, skipCount, neutralSafe, denseFx, pad;
+};
+
 struct DevPlan {
   DevColumn cols[kMaxPlanCols];
   DevInst insts[ARES_MAX_PLAN_INSTS];
@@ -94,6 +105,8 @@ struct DevPlan {
   uint8_t pad2[1];
   const DevJoin *join;     // device copy of the tables' indexes and the foreign columns' batches
   uint32_t resume;         // 1: relaunch of the same batch after the group table grew (DevTable::progress holds the resume points)
+  uint8_t nmeas;           // > 1: measure roots feeding that many states (direct-indexed form only); meas[] describes them
+  DevMeasure meas[kJitMaxMeasures];
 };
 
 constexpr uint32_t kDenseMaxSlots = 8192;   // = slots of a CTA's accumulator slice in AggState::ctaAcc

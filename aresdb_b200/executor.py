@@ -7,6 +7,8 @@
   engine, or (in tests / the CPU baseline) a HOST-mode build running on host memory.
 * `FusedBatchExecutor` is the B200-native form: one ExecuteBatchPlan call per batch into a
   device-resident AggState, one AggStateFinalize per query.
+* `FusedRequestExecutor` runs the queries of one AQL request: queries that share filters, dimensions and joins read each
+  batch once (ExecuteBatchPlanMulti, one state per query).
 
 Both take batches as lists of `VectorPartySlice`s that already live in the executor's memory space.
 """
@@ -325,23 +327,18 @@ class _PinnedPool:
 _PINNED = _PinnedPool()
 
 
-class FusedBatchExecutor:
-    """B200-native: one fused kernel per batch into a device-resident group table."""
+class _BatchPlans:
+    """The BatchPlan of a query's batches: instructions from `instructions(time_filters, cutoff)`, joined tables, and per
+    batch the columns, row count and zone map."""
 
-    def __init__(self, lib: A.Library, space, query: AggQuery, expected_groups: int = 0):
-        if not lib.has_plan_api:
-            raise RuntimeError("this library does not export the whole-batch plan API")
-        self.lib, self.space, self.q = lib, space, query
-        self.insts = query.plan_instructions()
-        self.state = C.c_void_p(lib.AggStateCreate(query.agg_spec(expected_groups), space.stream, space.device))
+    def __init__(self, query: AggQuery, instructions):
+        self.q, self._instructions = query, instructions
+        self.insts = instructions(True, 0)
         self._plan = A.BatchPlan()
         self._plan.NumInsts = len(self.insts)
         for i, pi in enumerate(self.insts):
             self._plan.Insts[i] = pi
         self._plan_variants = {}
-        self.calls = 0
-        self.skipped = 0   # batches whose zone map contradicts a filter (skipping.py): never launched
-        self.expected_groups = expected_groups
         # joined dimension tables: the lookup + foreign-column reads are a gather stage of the fused kernel
         self._join_keep = []
         if query.joins:
@@ -366,7 +363,7 @@ class FusedBatchExecutor:
         key = (time_filters, cutoff)
         p = self._plan_variants.get(key)
         if p is None:
-            insts = self.q.plan_instructions(time_filters=time_filters, cutoff=cutoff)
+            insts = self._instructions(time_filters, cutoff)
             p = A.BatchPlan()
             C.memmove(C.byref(p), C.byref(self._plan), C.sizeof(A.BatchPlan))   # foreign tables / columns as in the full plan
             p.NumInsts = len(insts)
@@ -377,13 +374,7 @@ class FusedBatchExecutor:
             self._plan_variants[key] = p
         return p
 
-    def process_batch(self, batch: Batch, stream=None, time_filters: bool = True, cutoff: int = 0):
-        """`time_filters=False`: an archive batch that lies strictly inside the query's time range skips the time filter
-        (archiveBatchCustomFilterExecutor evaluates it for the first and the last batch only, query/aql_processor.go:627-638).
-        `cutoff` > 0: a live batch of a fact table also evaluates `time >= cutoff` (liveBatchCustomFilterExecutor :543-567)."""
-        if should_skip_batch(self.q, batch.ranges):
-            self.skipped += 1
-            return
+    def plan_for(self, batch: Batch, time_filters: bool, cutoff: int) -> A.BatchPlan:
         lo, hi = self.q.time_filter_range
         p = self._plan if (time_filters or lo == hi) and cutoff <= 0 else self._plan_variant(time_filters or lo == hi, max(cutoff, 0))
         p.NumColumns = len(batch.columns)
@@ -396,6 +387,30 @@ class FusedBatchExecutor:
             r = batch.ranges.get(i) if batch.ranges else None
             p.Ranges[i].Known = 0 if r is None else 1
             p.Ranges[i].Min, p.Ranges[i].Max = (0, 0) if r is None else (int(r[0]), int(r[1]))
+        return p
+
+
+class FusedBatchExecutor:
+    """B200-native: one fused kernel per batch into a device-resident group table."""
+
+    def __init__(self, lib: A.Library, space, query: AggQuery, expected_groups: int = 0):
+        if not lib.has_plan_api:
+            raise RuntimeError("this library does not export the whole-batch plan API")
+        self.lib, self.space, self.q = lib, space, query
+        self.plans = _BatchPlans(query, lambda tf, co: query.plan_instructions(time_filters=tf, cutoff=co))
+        self.state = C.c_void_p(lib.AggStateCreate(query.agg_spec(expected_groups), space.stream, space.device))
+        self.calls = 0
+        self.skipped = 0   # batches whose zone map contradicts a filter (skipping.py): never launched
+        self.expected_groups = expected_groups
+
+    def process_batch(self, batch: Batch, stream=None, time_filters: bool = True, cutoff: int = 0):
+        """`time_filters=False`: an archive batch that lies strictly inside the query's time range skips the time filter
+        (archiveBatchCustomFilterExecutor evaluates it for the first and the last batch only, query/aql_processor.go:627-638).
+        `cutoff` > 0: a live batch of a fact table also evaluates `time >= cutoff` (liveBatchCustomFilterExecutor :543-567)."""
+        if should_skip_batch(self.q, batch.ranges):
+            self.skipped += 1
+            return
+        p = self.plans.plan_for(batch, time_filters, cutoff)
         self.calls += 1
         self.lib.ExecuteBatchPlan(self.state, C.byref(p), self.space.stream if stream is None else stream,
                                   self.space.device)
@@ -467,3 +482,70 @@ class FusedBatchExecutor:
             self.close()
         except Exception:
             pass
+
+
+MAX_SHARED_MEASURES = 4   # measure roots (states) of one ExecuteBatchPlanMulti plan
+
+
+def shared_scan_groups(queries: list) -> list[list[int]]:
+    """Indexes of `queries` grouped for one pass: queries with the same plan instructions except the measure root (same
+    filters in the same order, time-filter range, dimensions), the same joins and reduce mode, and no HLL; at most
+    MAX_SHARED_MEASURES per group, in request order.  Every other query is a group of its own."""
+    groups, open_group = [], {}
+    for i, q in enumerate(queries):
+        key = q.shared_scan_key()
+        g = open_group.get(key) if key is not None else None
+        if g is None or len(g) >= MAX_SHARED_MEASURES:
+            g = []
+            groups.append(g)
+            if key is not None:
+                open_group[key] = g
+        g.append(i)
+    return groups
+
+
+class FusedRequestExecutor:
+    """The queries of one AQL request (aql.compile_request): each keeps its own AggState and result, and the queries of a
+    compatible group (shared_scan_groups) read every batch once — one ExecuteBatchPlanMulti call whose plan carries one
+    measure root per query.  The engine picks the form per batch: one kernel for all of them, or each query's own kernel."""
+
+    def __init__(self, lib: A.Library, space, queries: list, expected_groups: int = 0):
+        self.lib, self.space, self.queries = lib, space, list(queries)
+        self.executors = [FusedBatchExecutor(lib, space, q, expected_groups) for q in self.queries]
+        self.groups = shared_scan_groups(self.queries)
+        self._shared = {}
+        for g in self.groups:
+            if len(g) > 1:
+                lead, members = self.queries[g[0]], [self.queries[i] for i in g]
+                self._shared[g[0]] = _BatchPlans(lead, lambda tf, co, lead=lead, members=members:
+                                                 lead.plan_instructions(time_filters=tf, cutoff=co, measures=members))
+        self.calls = 0
+
+    def process_batch(self, batch: Batch, stream=None, time_filters: bool = True, cutoff: int = 0):
+        """Same meaning as FusedBatchExecutor.process_batch, for every query of the request."""
+        for g in self.groups:
+            ex = self.executors[g[0]]
+            if len(g) == 1:
+                ex.process_batch(batch, stream, time_filters, cutoff)
+                continue
+            if should_skip_batch(ex.q, batch.ranges):   # (the group's filters are the same)
+                for i in g:
+                    self.executors[i].skipped += 1
+                continue
+            p = self._shared[g[0]].plan_for(batch, time_filters, cutoff)
+            states = (C.c_void_p * len(g))(*[self.executors[i].state.value for i in g])
+            self.calls += 1
+            self.lib.ExecuteBatchPlanMulti(states, len(g), C.byref(p), self.space.stream if stream is None else stream,
+                                           self.space.device)
+
+    def results(self) -> list:
+        """One QueryResult per query, in request order."""
+        return [ex.result() for ex in self.executors]
+
+    def reset(self):
+        for ex in self.executors:
+            ex.reset()
+
+    def close(self):
+        for ex in self.executors:
+            ex.close()

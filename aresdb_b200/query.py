@@ -125,10 +125,12 @@ class AggQuery:
         query/aql_processor.go:543-552; the time column of a fact table is column 0)."""
         return E.resolve(E.Binary(A.GreaterThanOrEqual, E.Col(self.time_column, A.Uint32, "time"), E.Lit(int(cutoff), E.Type.Unsigned)))
 
-    def plan_instructions(self, time_filters: bool = True, cutoff: int = 0) -> list[A.PlanInst]:
+    def plan_instructions(self, time_filters: bool = True, cutoff: int = 0, measures: list | None = None) -> list[A.PlanInst]:
         """Post-order flattening of every expression: one PlanInst per non-leaf AST node (what
         processExpression turns into one cgo call, reference query/time_series_aggregate.go:493-593).
-        `time_filters=False`: the plan of an archive batch strictly inside the query's time range."""
+        `time_filters=False`: the plan of an archive batch strictly inside the query's time range.
+        `measures`: queries sharing this query's filters and dimensions (shared_scan_key); the plan ends with their
+        measure roots, root k (SinkArg k) feeding the k-th state of ExecuteBatchPlanMulti."""
         insts: list[A.PlanInst] = []
         self.foreign_columns = []   # distinct (table, column, timezone) leaves in first-use order = BatchPlan.ForeignColumns
 
@@ -175,10 +177,22 @@ class AggQuery:
             emit(self.cutoff_filter(cutoff), A.PLAN_SINK_FILTER, 0, A.Bool)
         for pos, qi in enumerate(self.dim_order):
             emit(self.dimensions[qi], A.PLAN_SINK_DIMENSION, pos, self.dim_types[qi])
-        emit(self.measure, A.PLAN_SINK_MEASURE, 0, self.measure_data_type)
+        for k, q in enumerate([self] if measures is None else measures):
+            emit(q.measure, A.PLAN_SINK_MEASURE, k, q.measure_data_type)
         if len(insts) > A.ARES_MAX_PLAN_INSTS:
             raise ValueError("plan too long")
         return insts
+
+
+    def shared_scan_key(self):
+        """What queries must agree on to read the batches in one pass: the plan up to the measure root (filters in order,
+        with their literals, and dimensions), the time-filter positions, the joins and the reduce mode.  None for HLL
+        queries, which never share."""
+        if self.is_hll:
+            return None
+        prefix = tuple(bytes(pi) for pi in self.plan_instructions(measures=[]))
+        joins = tuple((id(j.table), j.on.index, j.timezone_ptr, j.timezone_size) for j in self.joins)
+        return prefix, self.time_filter_range, joins, self.reduce_mode
 
 
 class QueryResult:

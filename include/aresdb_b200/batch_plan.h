@@ -57,14 +57,15 @@ enum PlanSink {
   PLAN_SINK_STACK = 0,     /* non-root node: ScratchSpaceOutput of DataType SinkDataType       */
   PLAN_SINK_FILTER = 1,    /* root of a filter: row survives iff bool(value) (filterAction)      */
   PLAN_SINK_DIMENSION = 2, /* root of dimension #SinkArg (layout order), DimensionOutput         */
-  PLAN_SINK_MEASURE = 3    /* root of the measure, MeasureOutput of SinkDataType / AggSpec.AggFunc */
+  PLAN_SINK_MEASURE = 3    /* root of the measure, MeasureOutput of SinkDataType / AggSpec.AggFunc; ExecuteBatchPlanMulti:
+                            * one root per state, SinkArg = the ordinal of the state it feeds */
 };
 
 typedef struct {
   uint8_t NumOperands;  /* 1: Functor is a UnaryFunctorType; 2: a BinaryFunctorType */
   uint8_t Functor;
   uint8_t Sink;         /* enum PlanSink */
-  uint8_t SinkArg;      /* dimension ordinal for PLAN_SINK_DIMENSION */
+  uint8_t SinkArg;      /* dimension ordinal for PLAN_SINK_DIMENSION; state ordinal for PLAN_SINK_MEASURE (Multi) */
   uint8_t SinkDataType; /* enum DataType of the sink element */
   uint8_t Reserved[3];
   PlanOperand A;
@@ -155,6 +156,15 @@ CGoCallResHandle AggStateCreate(AggSpec spec, void *cudaStream, int device);
  * one stream at a time (the batches of a query follow each other, as in the reference); different states
  * run concurrently on different streams / devices. */
 CGoCallResHandle ExecuteBatchPlan(void *state, const BatchPlan *plan, void *cudaStream, int device);
+
+/* Several aggregates over the same rows in one pass: the plan carries numStates (1..4) PLAN_SINK_MEASURE roots, root
+ * SinkArg = k feeding states[k]; filters, dimensions and joins are shared.  Every state is an ordinary AggState
+ * (AggStateCreate; finalized, reset, exported and merged as usual); they must agree in NumDimsPerDimWidth and
+ * ReduceMode, and none may be AGGR_HLL.  When the batch's zone map lets every measure's own single-measure plan take the
+ * CTA's direct-indexed slots and they all fit a CTA together, one kernel evaluates each row once and feeds every state;
+ * otherwise each state runs its single-measure plan (what ExecuteBatchPlan would launch).  Results are the same either
+ * way.  numStates == 1 is ExecuteBatchPlan.  Asynchronous like ExecuteBatchPlan. */
+CGoCallResHandle ExecuteBatchPlanMulti(void *const *states, int numStates, const BatchPlan *plan, void *cudaStream, int device);
 
 /* Folds already-reduced rows (a DimensionVector block + measure vector, e.g. the carried
  * result of the legacy protocol, or the all-gathered results of other GPUs) into `state`
