@@ -357,6 +357,13 @@ _PLAN_SIGS = {
     "AggStateExportPartToPeers": [_VP, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_size_t, C.c_int, C.c_size_t,
                                   C.c_size_t, C.c_uint32, _VP, C.c_int],
     "AggStateMergePartsWhenFlagged": [_VP, _VP, C.c_int, C.c_size_t, C.c_int, C.c_size_t, C.c_size_t, _VP, C.c_uint32, _VP, C.c_int],
+    "AggStatesFinalize": [C.POINTER(C.c_void_p), C.c_int, C.POINTER(DimensionVector), C.POINTER(C.c_void_p), C.POINTER(C.c_int64), _VP,
+                          C.c_int],
+    "AggStatesExportPartsToPeers": [C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, C.c_int,
+                                    C.c_size_t, C.c_int, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t),
+                                    C.c_uint32, _VP, C.c_int],
+    "AggStatesMergeParts": [C.POINTER(C.c_void_p), C.c_int, _VP, C.c_int, C.c_size_t, C.c_int, C.POINTER(C.c_size_t),
+                            C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), _VP, C.c_uint32, _VP, C.c_int],
     "ComputeColumnRanges": [C.POINTER(VectorPartySlice), C.c_int, C.POINTER(ColumnRange), _VP, C.c_int],
 }
 _MEM_SIGS = {

@@ -19,6 +19,7 @@
 // merges equal hashes and writes the reference's output layout — the observable result of the
 // reference's Sort+Reduce (ARES_REDUCE_SORT) or HashReduce (ARES_REDUCE_HASH) over all batches.
 #include <cooperative_groups.h>
+#include <algorithm>
 #include <memory>
 #include <vector>
 
@@ -78,28 +79,53 @@ mergeRowsKernel(const uint8_t *__restrict__ block, DimLayout L, const uint8_t *_
     foldRow(block, L, measures, i, width, op, keyMode, hashBits, hll, G);
 }
 
-// Exchange step of a sharded query, receiving side: all N gathered parts ([groups, status, rows | dimension block of
-// `L.capacity` rows | measures]) are folded by ONE launch; the row counts are read from the parts' headers on the
-// device, so the host never waits for them.  A part whose sender could not fit its rows raises counters[2].  Parts carry no
-// HLL state (the export side refuses it).
-// `flags` != nullptr (exchange over peer memory, AggStateMergePartsWhenFlagged): the parts are written into this GPU's
-// memory by the PEERS' export kernels, each of which then stores `epoch` into flags[its rank] with release semantics at
-// system scope; every CTA waits for all numParts flags (acquire, system scope) before it reads a part.  The wait is
-// bounded (a peer that never arrives: counters[2], reported by finalize), so the kernel cannot hang the GPU.
-__global__ void __launch_bounds__(256)
-mergePartsKernel(const uint8_t *parts, int numParts, size_t partStride, size_t dimOff, size_t valOff, DimLayout L,
-                 int width, AggOp op, uint8_t keyMode, uint8_t hashBits, DevTable G, const uint32_t *flags, uint32_t epoch) {
+// States one exchange / finalize launch serves (AggStates*), and the flag stride of one state: a state's arrival flags are
+// 16 consecutive words (one per sending rank), the flags of state k start 16 * k words after those of state 0.
+constexpr int kMaxLaunchStates = 16;
+constexpr int kMaxPeers = 16;
+
+// Exchange step of a sharded request, receiving side: every state's N gathered parts ([groups, status, rows | dimension
+// block of `L.capacity` rows | measures]) are folded by ONE launch; blockIdx.y is the state, and the row counts are read
+// from the parts' headers on the device, so the host never waits for them.  Part p of state k lies at
+// slots + p * slotStride + partOff[k].  A part whose sender could not fit its rows raises counters[2] of ITS state only.
+// Parts carry no HLL state (the export side refuses it).
+// `flags` != nullptr (exchange over peer memory): the parts are written into this GPU's memory by the PEERS' export
+// kernels, each of which then stores `epoch` into flags[16 * k + its rank] with release semantics at system scope; every
+// CTA of state k waits for that state's numParts flags (acquire, system scope) before it reads a part, so no state waits
+// for another.  The wait is bounded (a peer that never arrives: counters[2] = 2, reported by finalize), so the kernel
+// cannot hang the GPU.
+struct MergeStateArgs {
+  DevTable G;
+  DimLayout L;
+  size_t partOff, dimOff, valOff;
+  int32_t width;
+  uint8_t op, keyMode, hashBits;
+};
+
+struct MergePartsArgs {
+  MergeStateArgs S[kMaxLaunchStates];
+  const uint8_t *slots;
+  size_t slotStride;
+  const uint32_t *flags;
+  int32_t numParts;
+  uint32_t epoch;
+};
+
+__global__ void __launch_bounds__(256) mergePartsKernel(const __grid_constant__ MergePartsArgs M) {
+  const MergeStateArgs &S = M.S[blockIdx.y];
+  const DevTable &G = S.G;
   const uint32_t stride = gridDim.x * blockDim.x;
-  if (flags != nullptr) {
+  if (M.flags != nullptr) {
+    const uint32_t *flags = M.flags + kMaxPeers * blockIdx.y;
     __shared__ uint32_t sLate;
     if (threadIdx.x == 0) {
       uint32_t late = 0;
       const long long t0 = clock64();
-      for (int p = 0; p < numParts && !late; p++) {
+      for (int p = 0; p < M.numParts && !late; p++) {
         for (;;) {
           uint32_t seen;
           asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(seen) : "l"(flags + p) : "memory");
-          if ((int32_t)(seen - epoch) >= 0) break;
+          if ((int32_t)(seen - M.epoch) >= 0) break;
           if (clock64() - t0 > 4000000000ll) { late = 1; break; }   // ~2 s at 2 GHz
           __nanosleep(100);
         }
@@ -110,17 +136,17 @@ mergePartsKernel(const uint8_t *parts, int numParts, size_t partStride, size_t d
     __syncthreads();
     if (sLate) return;
   }
-  for (int p = 0; p < numParts; p++) {
-    const uint8_t *part = parts + (size_t)p * partStride;
+  for (int p = 0; p < M.numParts; p++) {
+    const uint8_t *part = M.slots + (size_t)p * M.slotStride + S.partOff;
     const uint32_t *hdr = reinterpret_cast<const uint32_t *>(part);
     if (hdr[1] != SF_OK) {
       if (blockIdx.x == 0 && threadIdx.x == 0) atomicExch(&G.counters[2], 1u);
       continue;
     }
     const uint32_t n = hdr[0];
-    const uint8_t *block = part + dimOff, *measures = part + valOff;
+    const uint8_t *block = part + S.dimOff, *measures = part + S.valOff;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
-      foldRow(block, L, measures, i, width, op, keyMode, hashBits, 0, G);
+      foldRow(block, S.L, measures, i, S.width, (AggOp)S.op, S.keyMode, S.hashBits, 0, G);
   }
 }
 
@@ -441,11 +467,18 @@ __device__ __forceinline__ void exportClaimed(const SmallFinalizeArgs &A, uint32
   }
 }
 
-__global__ void __cluster_dims__(kFinCtas, 1, 1) __launch_bounds__(1024) finalizeSmallKernel(const __grid_constant__ SmallFinalizeArgs A) {
+// One launch serves several states: cluster c (CTAs c * kFinCtas ..) works on S[c] alone, with its own scratch and result
+// words, so clusters never wait for each other.
+struct SmallFinalizeBatch {
+  SmallFinalizeArgs S[kMaxLaunchStates];
+};
+
+__global__ void __cluster_dims__(kFinCtas, 1, 1) __launch_bounds__(1024, 1) finalizeSmallKernel(const __grid_constant__ SmallFinalizeBatch B) {
   __shared__ uint32_t off[kSmallBuckets + 1];
   __shared__ uint32_t sWarp[1024 / 32 + 1];
   cg::cluster_group cluster = cg::this_cluster();
   const uint32_t ctaRank = cluster.block_rank(), gtid = ctaRank * 1024u + threadIdx.x;
+  const SmallFinalizeArgs &A = B.S[blockIdx.x / kFinCtas];
   const DevTable &G = A.G;
   const uint32_t n = G.counters[0];
   uint32_t status = SF_OK;
@@ -558,23 +591,26 @@ __global__ void __cluster_dims__(kFinCtas, 1, 1) __launch_bounds__(1024) finaliz
   if (gtid == 0) publish(g, SF_OK, n);
 }
 
-// Exchange over peer memory, sending side: ONE kernel (a cluster of kFinCtas CTAs) writes this rank's rows as a part
-// ([rows, status, claimed | dimension block | measures], the layout of AggStateExportPart) into its own receive buffer,
-// copies the part into the same slot of every peer's receive buffer with 16-byte stores over NVLink, and then stores
-// `epoch` into flags[myRank] on every peer (release, system scope) — export, all-gather and the "it has arrived" signal
-// in one launch, no collective library and no host in between.
+// Exchange over peer memory, sending side: ONE kernel writes this rank's rows of every state as parts ([rows, status,
+// claimed | dimension block | measures], the layout of AggStateExportPart) into its own slot of its receive buffer —
+// cluster c (kFinCtas CTAs) exports state c into sub-part c —, copies each sub-part into the same place in every peer's
+// receive buffer with 16-byte stores over NVLink, and then stores `epoch` into state c's flag for this rank on every peer
+// (release, system scope) — export, all-gather and the "it has arrived" signal in one launch, no collective library and
+// no host in between.  peerFlag[0] == nullptr: the local export only (the parts then travel by a collective all-gather).
 struct PeerExportArgs {
-  SmallFinalizeArgs F;            // the export itself (ordered = 0); F.outBlock / F.outValues / F.resultDev lie in the local slot
-  uint8_t *peerSlot[16];          // this rank's slot in every peer's receive buffer (peerSlot[myRank]: the local one)
-  uint32_t *peerFlag[16];         // &flags[myRank] on every peer
-  size_t partBytes;               // multiple of 16
+  SmallFinalizeArgs F[kMaxLaunchStates];   // the exports (ordered = 0); outBlock / outValues / resultDev lie in the local sub-part
+  size_t partOffset[kMaxLaunchStates];     // sub-part of state c inside a slot
+  size_t partBytes[kMaxLaunchStates];      // its size, a multiple of 16
+  uint8_t *peerSlot[kMaxPeers];            // this rank's slot in every peer's receive buffer (peerSlot[myRank]: the local one)
+  uint32_t *peerFlag[kMaxPeers];           // &flags[state 0][myRank] on every peer; state c's flag lies kMaxPeers * c words further
   uint32_t numPeers, myRank, epoch;
 };
 
 __global__ void __cluster_dims__(kFinCtas, 1, 1) __launch_bounds__(1024) exportToPeersKernel(const __grid_constant__ PeerExportArgs E) {
   cg::cluster_group cluster = cg::this_cluster();
   const uint32_t gtid = cluster.block_rank() * 1024u + threadIdx.x;
-  const SmallFinalizeArgs &A = E.F;
+  const uint32_t c = blockIdx.x / kFinCtas;
+  const SmallFinalizeArgs &A = E.F[c];
   const DevTable &G = A.G;
   const uint32_t n = G.counters[0];
   uint32_t status = SF_OK;
@@ -583,19 +619,21 @@ __global__ void __cluster_dims__(kFinCtas, 1, 1) __launch_bounds__(1024) exportT
   else if (n > (uint32_t)A.outCapacity) status = SF_OUTPUT_TOO_SMALL;
   if (status == SF_OK) exportClaimed(A, n, gtid);
   if (gtid == 0) { A.resultDev[0] = status == SF_OK ? n : 0u; A.resultDev[1] = status; A.resultDev[2] = n; }
+  if (E.peerFlag[0] == nullptr) return;
   cluster.sync();   // the local part is complete (and visible to the cluster)
   // the part travels as it lies: header, the used prefix of every section would save bytes, but a part is 0.5 MB and the
   // copy is a few microseconds of NVLink time
-  const uint4 *src = reinterpret_cast<const uint4 *>(E.peerSlot[E.myRank]);
-  const uint32_t words = (uint32_t)(E.partBytes / 16);
+  const uint4 *src = reinterpret_cast<const uint4 *>(E.peerSlot[E.myRank] + E.partOffset[c]);
+  const uint32_t words = (uint32_t)(E.partBytes[c] / 16);
   for (uint32_t p = 0; p < E.numPeers; p++) {
     if (p == E.myRank) continue;
-    uint4 *dst = reinterpret_cast<uint4 *>(E.peerSlot[p]);
+    uint4 *dst = reinterpret_cast<uint4 *>(E.peerSlot[p] + E.partOffset[c]);
     for (uint32_t i = gtid; i < words; i += kFinThreads) dst[i] = src[i];
   }
   __threadfence_system();
   cluster.sync();   // every thread's stores are ordered before the flags
-  if (gtid < E.numPeers) asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(E.peerFlag[gtid]), "r"(E.epoch) : "memory");
+  if (gtid < E.numPeers)
+    asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(E.peerFlag[gtid] + kMaxPeers * c), "r"(E.epoch) : "memory");
 }
 
 // AggStateReset: only the claimed slots are emptied (and, for dense HLL states, only their register arrays).
@@ -1775,9 +1813,60 @@ static SmallFinalizeArgs smallFinalizeArgs(const AggState *st, int capacity, uin
   return A;
 }
 
-static int64_t finalize(AggState *st, const DimensionVector &out, uint8_t *outValues, cudaStream_t s, bool ordered = true) {
+// Launches the single-launch finalize / exchange-form export of n states: n clusters, cluster c on args[c].
+static void launchSmallFinalize(const SmallFinalizeArgs *args, int n, cudaStream_t s, const char *what) {
+  static thread_local SmallFinalizeBatch B;
+  for (int c = 0; c < n; c++) B.S[c] = args[c];
+  finalizeSmallKernel<<<kFinCtas * n, 1024, 0, s>>>(B);
+  checkLastError(what);
+}
+
+// The single-launch form takes states that announce at most kSmallFinalizeMax groups (their scratch is sized for it).
+static bool smallFinalizeFits(const AggState *st, const DimensionVector &out) {
+  return !st->hllDense && st->spec.ExpectedGroups <= (uint32_t)kSmallFinalizeMax && out.VectorCapacity > 0;
+}
+
+static SmallFinalizeArgs orderedFinalizeArgs(const AggState *st, const DimensionVector &out, uint8_t *outValues, bool ordered) {
+  SmallFinalizeArgs A = smallFinalizeArgs(st, out.VectorCapacity, out.DimValues, outValues, st->resultDev);
+  A.hashMask = testHash64Mask();
+  A.hashA = reinterpret_cast<uint64_t *>(st->smallScratch);
+  A.tmpK = A.hashA + kSmallFinalizeMax;
+  A.idxA = reinterpret_cast<uint32_t *>(A.tmpK + kSmallFinalizeMax);
+  A.tmpI = A.idxA + kSmallFinalizeMax;
+  A.hist = A.tmpI + kSmallFinalizeMax;
+  A.outHash = ordered ? out.HashValues : nullptr; A.outIndex = out.IndexVector;
+  A.resultHost = st->resultHostDev;
+  A.plusZero = st->spec.ReduceMode == ARES_REDUCE_HASH && (st->op == OP_SUM_F64 || st->op == OP_SUM_F32);
+  A.ordered = ordered;
+  return A;
+}
+
+static int64_t finalize(AggState *st, const DimensionVector &out, uint8_t *outValues, cudaStream_t s, bool ordered = true);
+static int64_t finalizeLarge(AggState *st, const DimensionVector &out, uint8_t *outValues, cudaStream_t s, bool ordered);
+
+// After the single-launch finalize of `st` and a synchronise: its group count, or the path that completes it.
+static int64_t finishSmallFinalize(AggState *st, const DimensionVector &out, uint8_t *outValues, cudaStream_t s, bool ordered) {
+  const uint32_t status = st->resultHost[1];
+  if (status == SF_UNSETTLED) {   // grow / fold the parked rows, then once more (the table moved: new pointers)
+    settleTable(st, s);
+    return finalize(st, out, outValues, s, ordered);
+  }
+  if (status == SF_OK) return st->resultHost[0];
+  if (status == SF_TABLE_OVERFLOW) checkOverflow(st, 1);
+  if (status == SF_OUTPUT_TOO_SMALL) throw EngineError("output DimensionVector capacity is smaller than the number of groups");
+  if (status == SF_PEER_LATE) throw EngineError("exchange over peer memory: a peer's part did not arrive within the wait bound");
+  if (status == SF_PART_TRUNCATED) throw EngineError("exchange part truncated: a rank held more rows than the fixed part carries; repeat the exchange with exact sizes");
+  // SF_TOO_MANY: more groups than one CTA sorts — the multi-launch path
+  return finalizeLarge(st, out, outValues, s, ordered);
+}
+
+static void checkOutputLayout(const AggState *st, const DimensionVector &out) {
   for (int i = 0; i < NUM_DIM_WIDTH; i++)
     if (out.NumDimsPerDimWidth[i] != st->spec.NumDimsPerDimWidth[i]) throw EngineError("dimension layout differs from AggSpec");
+}
+
+static int64_t finalize(AggState *st, const DimensionVector &out, uint8_t *outValues, cudaStream_t s, bool ordered) {
+  checkOutputLayout(st, out);
   if (st->hllDense) {  // carried rows straight from the register arrays (already in key order)
     DenseCarried dc;
     denseCarried(st, s, dc, false);
@@ -1792,36 +1881,49 @@ static int64_t finalize(AggState *st, const DimensionVector &out, uint8_t *outVa
     ARES_CUDA(cudaStreamSynchronize(s));
     return dc.entries;
   }
-  const int width = st->measWidth;
-  const bool plusZero = st->spec.ReduceMode == ARES_REDUCE_HASH && (st->op == OP_SUM_F64 || st->op == OP_SUM_F32);
-  if (st->spec.ExpectedGroups <= (uint32_t)kSmallFinalizeMax && out.VectorCapacity > 0) {
+  if (smallFinalizeFits(st, out)) {
     // results of up to 32768 groups: ONE launch (claim list -> hash -> sort -> merge -> emit) and ONE synchronise;
     // the group count comes back through mapped pinned memory
-    SmallFinalizeArgs A = smallFinalizeArgs(st, out.VectorCapacity, out.DimValues, outValues, st->resultDev);
-    A.hashMask = testHash64Mask();
-    A.hashA = reinterpret_cast<uint64_t *>(st->smallScratch);
-    A.tmpK = A.hashA + kSmallFinalizeMax;
-    A.idxA = reinterpret_cast<uint32_t *>(A.tmpK + kSmallFinalizeMax);
-    A.tmpI = A.idxA + kSmallFinalizeMax;
-    A.hist = A.tmpI + kSmallFinalizeMax;
-    A.outHash = ordered ? out.HashValues : nullptr; A.outIndex = out.IndexVector;
-    A.resultHost = st->resultHostDev;
-    A.plusZero = plusZero; A.ordered = ordered;
-    finalizeSmallKernel<<<kFinCtas, 1024, 0, s>>>(A);
-    checkLastError("finalizeSmall");
+    const SmallFinalizeArgs A = orderedFinalizeArgs(st, out, outValues, ordered);
+    launchSmallFinalize(&A, 1, s, "finalizeSmall");
     ARES_CUDA(cudaStreamSynchronize(s));
-    uint32_t status = st->resultHost[1];
-    if (status == SF_UNSETTLED) {   // grow / fold the parked rows, then once more (the table moved: new pointers)
-      settleTable(st, s);
-      return finalize(st, out, outValues, s, ordered);
-    }
-    if (status == SF_OK) return st->resultHost[0];
-    if (status == SF_TABLE_OVERFLOW) checkOverflow(st, 1);
-    if (status == SF_OUTPUT_TOO_SMALL) throw EngineError("output DimensionVector capacity is smaller than the number of groups");
-    if (status == SF_PEER_LATE) throw EngineError("exchange over peer memory: a peer's part did not arrive within the wait bound");
-    if (status == SF_PART_TRUNCATED) throw EngineError("exchange part truncated: a rank held more rows than the fixed part carries; repeat the exchange with exact sizes");
-    // SF_TOO_MANY: more groups than one CTA sorts — the multi-launch path below
+    return finishSmallFinalize(st, out, outValues, s, ordered);
   }
+  return finalizeLarge(st, out, outValues, s, ordered);
+}
+
+// AggStatesFinalize: every state that can takes ONE shared launch (one cluster each) and ONE synchronise; the others, and
+// those the launch could not finish (parked rows, more than kSmallFinalizeMax groups), complete through finalize's
+// paths.  groups[k] = the group count of state k, or -1 when it failed; the error then names every failed state.
+static void finalizeStates(AggState *const *sts, int numStates, const DimensionVector *outs, uint8_t *const *outValues, int64_t *groups,
+                           cudaStream_t s) {
+  SmallFinalizeArgs args[kMaxLaunchStates];
+  bool small[kMaxLaunchStates];
+  int m = 0;
+  for (int k = 0; k < numStates; k++) {
+    small[k] = smallFinalizeFits(sts[k], outs[k]);
+    if (small[k]) args[m++] = orderedFinalizeArgs(sts[k], outs[k], outValues[k], true);
+  }
+  if (m > 0) {
+    launchSmallFinalize(args, m, s, "AggStatesFinalize");
+    ARES_CUDA(cudaStreamSynchronize(s));
+  }
+  std::string failed;
+  for (int k = 0; k < numStates; k++) {
+    try {
+      groups[k] = small[k] ? finishSmallFinalize(sts[k], outs[k], outValues[k], s, true) : finalize(sts[k], outs[k], outValues[k], s);
+    } catch (const std::exception &e) {
+      groups[k] = -1;
+      failed += (failed.empty() ? "" : "\n") + std::string("state ") + std::to_string(k) + ": " + e.what();
+    }
+  }
+  if (!failed.empty()) throw EngineError(failed);
+}
+
+// The multi-launch finalize: results of more than kSmallFinalizeMax groups (or states that announce more).
+static int64_t finalizeLarge(AggState *st, const DimensionVector &out, uint8_t *outValues, cudaStream_t s, bool ordered) {
+  const int width = st->measWidth;
+  const bool plusZero = st->spec.ReduceMode == ARES_REDUCE_HASH && (st->op == OP_SUM_F64 || st->op == OP_SUM_F32);
   const int64_t occupied = groupCount(st, s);
   if (occupied == 0) return 0;
   const int n = (int)occupied;
@@ -1876,15 +1978,47 @@ static int64_t finalize(AggState *st, const DimensionVector &out, uint8_t *outVa
   return g;
 }
 
-// Folds the exchange parts (AggStateMergeParts / AggStateMergePartsWhenFlagged: `flags` != nullptr) with one launch.
-static void mergeParts(AggState *st, const char *fn, const uint8_t *parts, int numParts, size_t partStride, int capRows, size_t dimOffset,
-                       size_t valuesOffset, const uint32_t *flags, uint32_t epoch, cudaStream_t s) {
-  if (st->hll) throw EngineError(std::string(fn) + ": HLL states exchange through AggStateExport");
+// Folds the exchange parts of numStates states (AggState(s)MergeParts / AggStateMergePartsWhenFlagged: `flags` != nullptr)
+// with one launch.
+static void mergeParts(AggState *const *sts, int numStates, const char *fn, const uint8_t *slots, int numParts, size_t slotStride,
+                       int capRows, const size_t *partOffset, const size_t *dimOffset, const size_t *valuesOffset, const uint32_t *flags,
+                       uint32_t epoch, cudaStream_t s) {
+  for (int k = 0; k < numStates; k++)
+    if (sts[k]->hll) throw EngineError(std::string(fn) + ": HLL states exchange through AggStateExport");
   if (numParts <= 0) return;
-  ensureRoom(st, (uint64_t)numParts * (uint64_t)capRows, s);
-  DimLayout L = makeDimLayout(st->spec.NumDimsPerDimWidth, capRows);
-  mergePartsKernel<<<smCount() * 2, 256, 0, s>>>(parts, numParts, partStride, dimOffset, valuesOffset, L, st->measWidth, st->op,
-                                                 st->keyMode, (uint8_t)st->hashBits, st->table, flags, epoch);
+  static thread_local MergePartsArgs M;
+  memset(&M, 0, sizeof(M));
+  for (int k = 0; k < numStates; k++) {
+    AggState *st = sts[k];
+    ensureRoom(st, (uint64_t)numParts * (uint64_t)capRows, s);   // (may move the table: read it afterwards)
+    MergeStateArgs &S = M.S[k];
+    S.G = st->table;
+    S.L = makeDimLayout(st->spec.NumDimsPerDimWidth, capRows);
+    S.partOff = partOffset[k]; S.dimOff = dimOffset[k]; S.valOff = valuesOffset[k];
+    S.width = st->measWidth; S.op = (uint8_t)st->op; S.keyMode = (uint8_t)st->keyMode; S.hashBits = (uint8_t)st->hashBits;
+  }
+  M.slots = slots; M.slotStride = slotStride; M.flags = flags; M.numParts = numParts; M.epoch = epoch;
+  const int perState = smCount() * 2 / numStates;
+  mergePartsKernel<<<dim3(perState > 0 ? perState : 1, numStates), 256, 0, s>>>(M);
+  checkLastError(fn);
+}
+
+// Exchange-form export of numStates states into sub-parts of this rank's slot (peerSlots[myRank]) and, with peerFlags, the
+// copy into every peer's slot plus the arrival flags: one launch, asynchronous.
+static void exportPartsToPeers(AggState *const *sts, int numStates, uint8_t *const *peerSlots, uint32_t *const *peerFlags, int numPeers,
+                               int myRank, const size_t *partBytes, int capRows, const size_t *partOffset, const size_t *dimOffset,
+                               const size_t *valuesOffset, uint32_t epoch, cudaStream_t s, const char *fn) {
+  static thread_local PeerExportArgs E;
+  memset(&E, 0, sizeof(E));
+  for (int r = 0; r < numPeers; r++) { E.peerSlot[r] = peerSlots[r]; E.peerFlag[r] = peerFlags ? peerFlags[r] : nullptr; }
+  for (int k = 0; k < numStates; k++) {
+    uint8_t *part = peerSlots[myRank] + partOffset[k];
+    E.F[k] = smallFinalizeArgs(sts[k], capRows, part + dimOffset[k], part + valuesOffset[k], reinterpret_cast<uint32_t *>(part));
+    E.partOffset[k] = partOffset[k];
+    E.partBytes[k] = partBytes[k];
+  }
+  E.numPeers = (uint32_t)numPeers; E.myRank = (uint32_t)myRank; E.epoch = epoch;
+  exportToPeersKernel<<<kFinCtas * numStates, 1024, 0, s>>>(E);
   checkLastError(fn);
 }
 
@@ -2010,8 +2144,7 @@ CGoCallResHandle AggStateExportPart(void *state, uint8_t *part, int capRows, siz
     if (capRows <= 0 || capRows > kSmallFinalizeMax) throw EngineError("AggStateExportPart: capRows must be in [1, 32768]");
     SmallFinalizeArgs A = smallFinalizeArgs(st, capRows, part + dimOffset, part + valuesOffset, reinterpret_cast<uint32_t *>(part));
     A.resultHost = st->resultHostDev + 4;   // host copy unused
-    finalizeSmallKernel<<<kFinCtas, 1024, 0, (cudaStream_t)cudaStream>>>(A);
-    checkLastError("AggStateExportPart");
+    launchSmallFinalize(&A, 1, (cudaStream_t)cudaStream, "AggStateExportPart");
     return 0;
   });
 }
@@ -2021,7 +2154,9 @@ CGoCallResHandle AggStateExportPart(void *state, uint8_t *part, int capRows, siz
 CGoCallResHandle AggStateMergeParts(void *state, const uint8_t *parts, int numParts, size_t partStride, int capRows,
                                     size_t dimOffset, size_t valuesOffset, void *cudaStream, int device) {
   return guarded("AggStateMergeParts", device, [&]() -> int64_t {
-    mergeParts(asState(state), "AggStateMergeParts", parts, numParts, partStride, capRows, dimOffset, valuesOffset, nullptr, 0u,
+    AggState *st = asState(state);
+    const size_t partOffset = 0;
+    mergeParts(&st, 1, "AggStateMergeParts", parts, numParts, partStride, capRows, &partOffset, &dimOffset, &valuesOffset, nullptr, 0u,
                (cudaStream_t)cudaStream);
     return 0;
   });
@@ -2039,14 +2174,9 @@ CGoCallResHandle AggStateExportPartToPeers(void *state, uint8_t *const *peerSlot
     if (capRows <= 0 || capRows > kSmallFinalizeMax) throw EngineError("AggStateExportPartToPeers: capRows must be in [1, 32768]");
     if (numPeers <= 0 || numPeers > 16 || myRank < 0 || myRank >= numPeers) throw EngineError("AggStateExportPartToPeers: 1..16 peers");
     if (partBytes % 16 != 0) throw EngineError("AggStateExportPartToPeers: partBytes must be a multiple of 16");
-    PeerExportArgs E;
-    memset(&E, 0, sizeof(E));
-    for (int r = 0; r < numPeers; r++) { E.peerSlot[r] = peerSlots[r]; E.peerFlag[r] = peerFlags[r]; }
-    uint8_t *part = peerSlots[myRank];
-    E.F = smallFinalizeArgs(st, capRows, part + dimOffset, part + valuesOffset, reinterpret_cast<uint32_t *>(part));
-    E.partBytes = partBytes; E.numPeers = (uint32_t)numPeers; E.myRank = (uint32_t)myRank; E.epoch = epoch;
-    exportToPeersKernel<<<kFinCtas, 1024, 0, (cudaStream_t)cudaStream>>>(E);
-    checkLastError("AggStateExportPartToPeers");
+    const size_t partOffset = 0;
+    exportPartsToPeers(&st, 1, peerSlots, peerFlags, numPeers, myRank, &partBytes, capRows, &partOffset, &dimOffset, &valuesOffset, epoch,
+                       (cudaStream_t)cudaStream, "AggStateExportPartToPeers");
     return 0;
   });
 }
@@ -2058,7 +2188,100 @@ CGoCallResHandle AggStateMergePartsWhenFlagged(void *state, const uint8_t *parts
                                                void *cudaStream, int device) {
   return guarded("AggStateMergePartsWhenFlagged", device, [&]() -> int64_t {
     if (flags == nullptr) throw EngineError("AggStateMergePartsWhenFlagged: flags is null");
-    mergeParts(asState(state), "AggStateMergePartsWhenFlagged", parts, numParts, partStride, capRows, dimOffset, valuesOffset, flags,
+    AggState *st = asState(state);
+    const size_t partOffset = 0;
+    mergeParts(&st, 1, "AggStateMergePartsWhenFlagged", parts, numParts, partStride, capRows, &partOffset, &dimOffset, &valuesOffset,
+               flags, epoch, (cudaStream_t)cudaStream);
+    return 0;
+  });
+}
+
+// ---- several states per launch (the queries of one request) ----
+// The states of one call: 1..kMaxLaunchStates distinct, non-HLL AggStates.
+static void requestStates(void *const *states, int numStates, AggState **sts) {
+  if (states == nullptr) throw EngineError("states is null");
+  if (numStates < 1 || numStates > kMaxLaunchStates) throw EngineError("numStates must be 1.." + std::to_string(kMaxLaunchStates));
+  for (int k = 0; k < numStates; k++) {
+    sts[k] = asState(states[k]);
+    if (sts[k]->hll) throw EngineError("state " + std::to_string(k) + " is AGGR_HLL: HLL states exchange through AggStateExport");
+    for (int j = 0; j < k; j++)
+      if (sts[j] == sts[k]) throw EngineError("state " + std::to_string(k) + " appears twice");
+  }
+}
+
+// Checks the per-state sub-part layout of an exchange slot: 16-byte aligned offsets, the header in front of the dimension
+// block, the dimension block in front of the measures, every sub-part inside the slot and no two overlapping.  Returns
+// each sub-part's size (a multiple of 16) in partBytes.
+static void checkSlotLayout(AggState *const *sts, int numStates, size_t slotBytes, int capRows, const size_t *partOffset,
+                            const size_t *dimOffset, const size_t *valuesOffset, size_t *partBytes) {
+  if (!partOffset || !dimOffset || !valuesOffset) throw EngineError("partOffset / dimOffset / valuesOffset must not be null");
+  if (capRows <= 0 || capRows > kSmallFinalizeMax) throw EngineError("capRows must be in [1, 32768]");
+  if (slotBytes % 16 != 0) throw EngineError("slotBytes must be a multiple of 16");
+  for (int k = 0; k < numStates; k++) {
+    const std::string who = "state " + std::to_string(k) + ": ";
+    if (partOffset[k] % 16 || dimOffset[k] % 16 || valuesOffset[k] % 16) throw EngineError(who + "offsets must be multiples of 16");
+    const DimLayout L = makeDimLayout(sts[k]->spec.NumDimsPerDimWidth, capRows);
+    size_t dimBytes = 0;
+    for (int d = 0; d < L.numDims; d++) dimBytes = std::max<size_t>(dimBytes, (size_t)L.nullOff[d] + (size_t)capRows);
+    if (dimOffset[k] < 16 || valuesOffset[k] < dimOffset[k] + dimBytes)
+      throw EngineError(who + "the header (16 bytes), the dimension block and the measures must follow each other");
+    partBytes[k] = (valuesOffset[k] + (size_t)sts[k]->measWidth * (size_t)capRows + 15) / 16 * 16;
+    if (partOffset[k] > slotBytes || partBytes[k] > slotBytes - partOffset[k]) throw EngineError(who + "the sub-part does not fit the slot");
+    for (int j = 0; j < k; j++)
+      if (partOffset[j] < partOffset[k] + partBytes[k] && partOffset[k] < partOffset[j] + partBytes[j])
+        throw EngineError(who + "the sub-part overlaps that of state " + std::to_string(j));
+  }
+}
+
+CGoCallResHandle AggStatesFinalize(void *const *states, int numStates, const DimensionVector *outputKeys, uint8_t *const *outputValues,
+                                   int64_t *groups, void *cudaStream, int device) {
+  return guarded("AggStatesFinalize", device, [&]() -> int64_t {
+    AggState *sts[kMaxLaunchStates];
+    requestStates(states, numStates, sts);
+    if (!outputKeys || !outputValues || !groups) throw EngineError("outputKeys / outputValues / groups must not be null");
+    for (int k = 0; k < numStates; k++) {
+      try {
+        checkOutputLayout(sts[k], outputKeys[k]);
+      } catch (const EngineError &e) {
+        throw EngineError("state " + std::to_string(k) + ": " + e.what());
+      }
+    }
+    finalizeStates(sts, numStates, outputKeys, outputValues, groups, (cudaStream_t)cudaStream);
+    return 0;
+  });
+}
+
+CGoCallResHandle AggStatesExportPartsToPeers(void *const *states, int numStates, uint8_t *const *peerSlots, uint32_t *const *peerFlags,
+                                             int numPeers, int myRank, size_t slotBytes, int capRows, const size_t *partOffset,
+                                             const size_t *dimOffset, const size_t *valuesOffset, uint32_t epoch, void *cudaStream,
+                                             int device) {
+  return guarded("AggStatesExportPartsToPeers", device, [&]() -> int64_t {
+    AggState *sts[kMaxLaunchStates];
+    requestStates(states, numStates, sts);
+    if (!peerSlots) throw EngineError("peerSlots is null");
+    if (numPeers < 1 || numPeers > kMaxPeers || myRank < 0 || myRank >= numPeers)
+      throw EngineError("numPeers must be 1..16 and myRank < numPeers");
+    size_t partBytes[kMaxLaunchStates];
+    checkSlotLayout(sts, numStates, slotBytes, capRows, partOffset, dimOffset, valuesOffset, partBytes);
+    for (int r = 0; r < numPeers; r++)
+      if ((r == myRank || peerFlags) && (!peerSlots[r] || (peerFlags && !peerFlags[r]))) throw EngineError("null peer slot or flag");
+    exportPartsToPeers(sts, numStates, peerSlots, peerFlags, numPeers, myRank, partBytes, capRows, partOffset, dimOffset, valuesOffset,
+                       epoch, (cudaStream_t)cudaStream, "AggStatesExportPartsToPeers");
+    return 0;
+  });
+}
+
+CGoCallResHandle AggStatesMergeParts(void *const *states, int numStates, const uint8_t *slots, int numParts, size_t slotStride, int capRows,
+                                     const size_t *partOffset, const size_t *dimOffset, const size_t *valuesOffset, const uint32_t *flags,
+                                     uint32_t epoch, void *cudaStream, int device) {
+  return guarded("AggStatesMergeParts", device, [&]() -> int64_t {
+    AggState *sts[kMaxLaunchStates];
+    requestStates(states, numStates, sts);
+    if (!slots) throw EngineError("slots is null");
+    if (numParts < 1 || numParts > kMaxPeers) throw EngineError("numParts must be 1..16");
+    size_t partBytes[kMaxLaunchStates];
+    checkSlotLayout(sts, numStates, slotStride, capRows, partOffset, dimOffset, valuesOffset, partBytes);
+    mergeParts(sts, numStates, "AggStatesMergeParts", slots, numParts, slotStride, capRows, partOffset, dimOffset, valuesOffset, flags,
                epoch, (cudaStream_t)cudaStream);
     return 0;
   });

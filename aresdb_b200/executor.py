@@ -15,6 +15,7 @@ Both take batches as lists of `VectorPartySlice`s that already live in the execu
 from __future__ import annotations
 
 import ctypes as C
+import re
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -441,10 +442,7 @@ class FusedBatchExecutor:
                 cap = max(self.group_count(), 1)
 
     def result(self) -> QueryResult:
-        g, out = self.finalize_into()
-        if g == 0:
-            return QueryResult(self.q, np.zeros(0, np.uint8), 1, np.zeros(0, np.uint8), 0)
-        return QueryResult(self.q, out.dims.get(np.uint8), out.capacity, out.measures.get(np.uint8), g)
+        return query_result(self.q, *self.finalize_into())
 
     def hll_result(self) -> HLLResult:
         """hll queries: the register vectors of every dimension group (AggStateFinalizeHLL)."""
@@ -484,6 +482,61 @@ class FusedBatchExecutor:
             pass
 
 
+def query_result(q: AggQuery, g: int, out: _ResultBuffers) -> QueryResult:
+    """The QueryResult of `g` groups finalized into `out`."""
+    if g == 0:
+        return QueryResult(q, np.zeros(0, np.uint8), 1, np.zeros(0, np.uint8), 0)
+    return QueryResult(q, out.dims.get(np.uint8), out.capacity, out.measures.get(np.uint8), g)
+
+
+MAX_LAUNCH_STATES = 16   # states of one AggStatesFinalize / AggStatesExportPartsToPeers / AggStatesMergeParts call
+
+
+def finalize_states(executors: list) -> list:
+    """finalize_into of every executor (non-HLL queries) with one AggStatesFinalize per MAX_LAUNCH_STATES states: those
+    that announce at most SMALL_RESULT groups share one launch and one synchronise.  Per executor: (groups,
+    _ResultBuffers), or the AresError of a state whose finalize failed while the others completed."""
+    done = []
+    for i in range(0, len(executors), MAX_LAUNCH_STATES):
+        done += _finalize_some(executors[i:i + MAX_LAUNCH_STATES])
+    return done
+
+
+def _finalize_some(exs: list) -> list:
+    if not exs:
+        return []
+    lib, sp, n = exs[0].lib, exs[0].space, len(exs)
+    bufs = []
+    for ex in exs:   # (capacity as finalize_into's first attempt)
+        cap = ex.SMALL_RESULT if ex.expected_groups <= ex.SMALL_RESULT else max(ex.group_count(), 1)
+        bufs.append(_ResultBuffers(sp, ex.q, cap, zero=not getattr(sp, "is_cuda", False)))
+    states = (C.c_void_p * n)(*[ex.state.value for ex in exs])
+    keys = (A.DimensionVector * n)(*[b.dimension_vector(ex.q) for b, ex in zip(bufs, exs)])
+    values = (C.c_void_p * n)(*[b.measures.ptr for b in bufs])
+    groups = (C.c_int64 * n)(*([-2] * n))
+    failed = {}
+    try:
+        lib.AggStatesFinalize(states, n, keys, values, groups, sp.stream, sp.device)
+    except A.AresError as e:
+        # per-state failures: one line "state k: <message>" each, groups[k] = -1; anything else failed the whole call
+        for line in str(e).removeprefix("AggStatesFinalize: ").split("\n"):
+            m = re.match(r"state (\d+): (.*)", line)
+            if m is None or groups[int(m.group(1))] != -1:
+                raise
+            failed[int(m.group(1))] = A.AresError(m.group(2))
+        if any(g == -2 for g in groups):
+            raise
+    done = []
+    for k, ex in enumerate(exs):
+        if k not in failed:
+            done.append((groups[k], bufs[k]))
+        elif "capacity is smaller" in str(failed[k]):
+            done.append(ex.finalize_into(max(ex.group_count(), 1)))   # finalize_into's second attempt: the exact count
+        else:
+            done.append(failed[k])
+    return done
+
+
 MAX_SHARED_MEASURES = 4   # measure roots (states) of one ExecuteBatchPlanMulti plan
 
 
@@ -509,9 +562,11 @@ class FusedRequestExecutor:
     compatible group (shared_scan_groups) read every batch once — one ExecuteBatchPlanMulti call whose plan carries one
     measure root per query.  The engine picks the form per batch: one kernel for all of them, or each query's own kernel."""
 
-    def __init__(self, lib: A.Library, space, queries: list, expected_groups: int = 0):
+    def __init__(self, lib: A.Library, space, queries: list, expected_groups: int | list = 0):
+        """`expected_groups`: one hint for every query, or a list with one per query."""
         self.lib, self.space, self.queries = lib, space, list(queries)
-        self.executors = [FusedBatchExecutor(lib, space, q, expected_groups) for q in self.queries]
+        eg = list(expected_groups) if isinstance(expected_groups, (list, tuple)) else [expected_groups] * len(self.queries)
+        self.executors = [FusedBatchExecutor(lib, space, q, g) for q, g in zip(self.queries, eg)]
         self.groups = shared_scan_groups(self.queries)
         self._shared = {}
         for g in self.groups:
@@ -539,8 +594,19 @@ class FusedRequestExecutor:
                                            self.space.device)
 
     def results(self) -> list:
-        """One QueryResult per query, in request order."""
-        return [ex.result() for ex in self.executors]
+        """One QueryResult per query, in request order.  The non-HLL queries are finalized together (one AggStatesFinalize
+        launch and one synchronise for those that announce at most SMALL_RESULT groups)."""
+        idx = [i for i, q in enumerate(self.queries) if not q.is_hll]
+        done = dict(zip(idx, finalize_states([self.executors[i] for i in idx])))
+        out = []
+        for i, ex in enumerate(self.executors):
+            if i not in done:
+                out.append(ex.result())
+            elif isinstance(done[i], Exception):
+                raise done[i]
+            else:
+                out.append(query_result(ex.q, *done[i]))
+        return out
 
     def reset(self):
         for ex in self.executors:

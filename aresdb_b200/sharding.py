@@ -8,11 +8,19 @@ with the aggregate's combine rule — what the reference's broker does with JSON
 """
 from __future__ import annotations
 
+import ctypes as C
+import os
+import sys
+
 import numpy as np
 
 from . import cabi as A
-from .executor import _ResultBuffers, dim_offsets
+from .executor import MAX_LAUNCH_STATES, _ResultBuffers, dim_offsets, finalize_states, query_result
 from .query import AggQuery, QueryResult
+
+
+EXCHANGE_ROWS = 32768   # rows of a fixed part (= what the engine's single-launch export handles)
+_PART_HDR = 64          # a part's header (16 bytes used) in front of its dimension block
 
 
 def assign_batches(num_batches: int, world: int, rank: int) -> list[int]:
@@ -62,8 +70,8 @@ class ShardedFusedQuery:
     def process_batch(self, batch, stream=None):
         self.local.process_batch(batch, stream)
 
-    EXCHANGE_ROWS = 32768   # rows of a fixed part (= what the engine's single-launch export handles)
-    _HDR = 64
+    EXCHANGE_ROWS = EXCHANGE_ROWS
+    _HDR = _PART_HDR
 
     def _exchange_fixed(self):
         """Device-only exchange: AggStateExportPart (one launch, the row count stays on the device) -> ONE all-gather of
@@ -92,30 +100,10 @@ class ShardedFusedQuery:
     _FLAGS = 256   # two parities x 16 ranks x uint32, in front of the two receive buffers
 
     def _setup_peers(self, part: int):
-        """Maps every rank's receive buffer into every process (torch symmetric memory: CUDA IPC / fabric handles over
-        NVLink) for the exchange over peer memory.  All ranks agree on the outcome; on failure the NCCL all-gather stays."""
-        import os
-        import sys
-        import torch
-        ok = 0
-        if os.environ.get("ARESDB_B200_EXCHANGE", "peer") == "peer" and self.world <= 16:
-            try:
-                import torch.distributed._symmetric_memory as symm
-                buf = symm.empty(self._FLAGS + 2 * self.world * part, dtype=torch.uint8, device=self.space.dev)
-                buf.zero_()
-                hdl = symm.rendezvous(buf, self.dist.group.WORLD)
-                ptrs = [int(p) for p in hdl.buffer_ptrs]
-                torch.cuda.synchronize()
-                self._peer = dict(buf=buf, hdl=hdl, ptrs=ptrs, epoch=0, part=part)
-                ok = 1
-            except Exception as e:   # no peer access between these GPUs, or a torch without symmetric memory
-                print(f"[aresdb_b200] exchange over peer memory unavailable ({type(e).__name__}: {e}); using the NCCL all-gather",
-                      file=sys.stderr)
-        agree = torch.tensor([ok], device=self.space.dev, dtype=torch.int32)
-        self.dist.all_reduce(agree, op=self.dist.ReduceOp.MIN)   # (also: nobody writes before everybody has zeroed its flags)
-        self._peer_ok = bool(agree.item())
-        if not self._peer_ok:
-            self._peer = None
+        self._peer = setup_peer_buffers(self.dist, self.space, self.world, self._FLAGS + 2 * self.world * part)
+        self._peer_ok = self._peer is not None
+        if self._peer is not None:
+            self._peer["part"] = part
 
     def _exchange_peers(self, cap: int, dim_bytes: int):
         """AggStateExportPartToPeers (ONE launch: export + copy of the part into every peer's receive buffer over NVLink +
@@ -141,35 +129,8 @@ class ShardedFusedQuery:
         return self._exchange_exact()
 
     def _exchange_exact(self):
-        """The one exchange step: every rank exports its table (AggStateExport: unordered rows, no
-        sort), ONE all-gather moves [dim block | measure vector] of every rank, and every rank folds
-        all of them into `self.merged`.  Returns the number of rows gathered (an upper bound of the
-        merged group count).  For hll queries the rows are the carried (group, register) entries."""
-        import torch
-        q, sp, dist, lib = self.q, self.space, self.dist, self.lib
-        n = self.local.group_count()
-        counts = torch.zeros(self.world, dtype=torch.int64, device=sp.dev)
-        counts[self.rank] = n
-        dist.all_reduce(counts)
-        counts = counts.tolist()
-        cap = max(max(counts), 1)
-        _, _, _, dim_bytes = dim_offsets(q.num_dims_per_width, cap)
-        dim_bytes = (dim_bytes + 15) // 16 * 16
-        part = dim_bytes + q.measure_bytes * cap
-        gathered = torch.empty(self.world * part, dtype=torch.uint8, device=sp.dev)
-        mine = gathered[self.rank * part:(self.rank + 1) * part]
-        if n:
-            dv = A.make_dimension_vector(mine.data_ptr(), None, None, q.num_dims_per_width, cap)
-            lib.AggStateExport(self.local.state, dv, mine.data_ptr() + dim_bytes, sp.stream, sp.device)
-        dist.all_gather_into_tensor(gathered, mine.clone())
-        self.merged.reset()
-        base = gathered.data_ptr()
-        for r in range(self.world):
-            if counts[r]:
-                dv = A.make_dimension_vector(base + r * part, None, None, q.num_dims_per_width, cap)
-                self.merged.merge(dv, base + r * part + dim_bytes, counts[r])
-        self._keep = gathered   # merge is asynchronous: keep the gathered rows alive until finalize
-        return int(sum(counts))
+        rows, self._keep = exchange_exact(self.dist, self.world, self.rank, self.local, self.merged)
+        return rows
 
     def finalize(self):
         """(groups, result buffers) of the WHOLE query, identical on every rank."""
@@ -195,6 +156,195 @@ class ShardedFusedQuery:
         self.local.close()
         if self.merged:
             self.merged.close()
+
+
+def setup_peer_buffers(dist, space, world: int, nbytes: int):
+    """Maps every rank's receive buffer of `nbytes` into every process (torch symmetric memory: CUDA IPC / fabric handles
+    over NVLink) for the exchange over peer memory: dict(buf, hdl, ptrs, epoch=0), or None.  All ranks agree on the
+    outcome; on failure (or with ARESDB_B200_EXCHANGE other than "peer") the NCCL all-gather stays."""
+    import torch
+    ok, peer = 0, None
+    if os.environ.get("ARESDB_B200_EXCHANGE", "peer") == "peer" and world <= 16:
+        try:
+            import torch.distributed._symmetric_memory as symm
+            buf = symm.empty(nbytes, dtype=torch.uint8, device=space.dev)
+            buf.zero_()
+            hdl = symm.rendezvous(buf, dist.group.WORLD)
+            ptrs = [int(p) for p in hdl.buffer_ptrs]
+            torch.cuda.synchronize()
+            peer = dict(buf=buf, hdl=hdl, ptrs=ptrs, epoch=0)
+            ok = 1
+        except Exception as e:   # no peer access between these GPUs, or a torch without symmetric memory
+            print(f"[aresdb_b200] exchange over peer memory unavailable ({type(e).__name__}: {e}); using the NCCL all-gather",
+                  file=sys.stderr)
+    agree = torch.tensor([ok], device=space.dev, dtype=torch.int32)
+    dist.all_reduce(agree, op=dist.ReduceOp.MIN)   # (also: nobody writes before everybody has zeroed its flags)
+    return peer if agree.item() else None
+
+
+def exchange_exact(dist, world: int, rank: int, local, merged):
+    """The exact-size exchange step of one query: every rank exports its table (AggStateExport: unordered rows, no sort),
+    ONE all-gather moves [dim block | measure vector] of every rank, and every rank folds all of them into `merged` (a
+    FusedBatchExecutor, reset first).  Returns (rows gathered — an upper bound of the merged group count —, the gathered
+    tensor, which must stay alive until the merged state is finalized).  For hll queries the rows are the carried (group,
+    register) entries."""
+    import torch
+    q, sp, lib = local.q, local.space, local.lib
+    n = local.group_count()
+    counts = torch.zeros(world, dtype=torch.int64, device=sp.dev)
+    counts[rank] = n
+    dist.all_reduce(counts)
+    counts = counts.tolist()
+    cap = max(max(counts), 1)
+    _, _, _, dim_bytes = dim_offsets(q.num_dims_per_width, cap)
+    dim_bytes = (dim_bytes + 15) // 16 * 16
+    part = dim_bytes + q.measure_bytes * cap
+    gathered = torch.empty(world * part, dtype=torch.uint8, device=sp.dev)
+    mine = gathered[rank * part:(rank + 1) * part]
+    if n:
+        dv = A.make_dimension_vector(mine.data_ptr(), None, None, q.num_dims_per_width, cap)
+        lib.AggStateExport(local.state, dv, mine.data_ptr() + dim_bytes, sp.stream, sp.device)
+    dist.all_gather_into_tensor(gathered, mine.clone())
+    merged.reset()
+    base = gathered.data_ptr()
+    for r in range(world):
+        if counts[r]:
+            dv = A.make_dimension_vector(base + r * part, None, None, q.num_dims_per_width, cap)
+            merged.merge(dv, base + r * part + dim_bytes, counts[r])
+    return int(sum(counts)), gathered
+
+
+def request_slot_layout(queries: list, cap_rows: int = EXCHANGE_ROWS):
+    """One rank's exchange slot of a request: per query a sub-part [header | dimension block of `cap_rows` rows |
+    measures], each sized from the query's dimensions and measure width and 16-byte aligned.  Returns (part offsets,
+    dimension-block offsets, measure offsets — the last two relative to their sub-part —, slot bytes)."""
+    parts, dims, values, pos = [], [], [], 0
+    for q in queries:
+        _, _, _, dim_bytes = dim_offsets(q.num_dims_per_width, cap_rows)
+        dim_bytes = (dim_bytes + 15) // 16 * 16
+        parts.append(pos)
+        dims.append(_PART_HDR)
+        values.append(_PART_HDR + dim_bytes)
+        pos += (_PART_HDR + dim_bytes + q.measure_bytes * cap_rows + 15) // 16 * 16
+    return parts, dims, values, (pos + 63) // 64 * 64
+
+
+class ShardedFusedRequest:
+    """One rank's half of a sharded AQL request (torch.distributed / NCCL plumbing).  The rank's batches are scanned by a
+    FusedRequestExecutor, so queries that share filters and dimensions share the scan on every rank.  finalize() exchanges
+    every non-HLL query that announces at most EXCHANGE_ROWS groups in ONE export launch (the rank's slot holds one
+    sub-part per query; over peer memory when every rank can map every other's receive buffer, else one NCCL all-gather
+    — ARESDB_B200_EXCHANGE as for ShardedFusedQuery), folds them with ONE merge launch and finalizes them with ONE
+    AggStatesFinalize.  HLL queries, queries that announce more groups and queries whose sub-part was truncated take the
+    exact-size protocol (exchange_exact)."""
+
+    _FLAGS_PER_PARITY = MAX_LAUNCH_STATES * 16 * 4   # uint32 flags[state][16 ranks] of one epoch parity
+
+    def __init__(self, lib, space, queries: list, expected_groups: int | list = 0):
+        """`expected_groups`: one hint for every query, or a list with one per query."""
+        from .executor import FusedBatchExecutor, FusedRequestExecutor
+        queries = list(queries)
+        if not queries or len(queries) > MAX_LAUNCH_STATES:
+            raise ValueError(f"a sharded request holds 1..{MAX_LAUNCH_STATES} queries, not {len(queries)}")
+        if not all(isinstance(q, AggQuery) for q in queries):
+            raise TypeError("every query of a sharded request must be an AggQuery")
+        eg = list(expected_groups) if isinstance(expected_groups, (list, tuple)) else [expected_groups] * len(queries)
+        if len(eg) != len(queries) or not all(isinstance(g, int) and not isinstance(g, bool) and g >= 0 for g in eg):
+            raise ValueError("expected_groups must be a non-negative int, or one per query")
+        import torch.distributed as dist
+        self.dist = dist
+        self.world = dist.get_world_size() if dist.is_initialized() else 1
+        self.rank = dist.get_rank() if dist.is_initialized() else 0
+        self.lib, self.space, self.queries = lib, space, queries
+        self.local = FusedRequestExecutor(lib, space, queries, eg)
+        self.merged = [FusedBatchExecutor(lib, space, q, g) for q, g in zip(queries, eg)] if self.world > 1 else None
+        fixed_ok = self.world > 1 and os.environ.get("ARESDB_B200_EXCHANGE", "fixed") != "exact"
+        self.fixed = [i for i, q in enumerate(queries) if fixed_ok and not q.is_hll and eg[i] <= EXCHANGE_ROWS]
+        self._layout = request_slot_layout([queries[i] for i in self.fixed])
+        self._send = self._recv = None
+        self._peer, self._peer_ok = None, None   # exchange over peer memory: set up at the first exchange
+        self._merged_dirty = False
+        self._keep = []
+
+    def process_batch(self, batch, stream=None, time_filters: bool = True, cutoff: int = 0):
+        """Same meaning as FusedRequestExecutor.process_batch (archive.scan_shard drives a rank's share with it)."""
+        self.local.process_batch(batch, stream, time_filters, cutoff)
+
+    def reset(self):
+        self.local.reset()
+
+    def _exchange_fixed(self):
+        """Export (one launch) -> peer copy or one all-gather -> merge (one launch) of the fixed-exchange queries."""
+        import torch
+        sp, lib, w, r = self.space, self.lib, self.world, self.rank
+        parts, dims, values, slot = self._layout
+        k = len(self.fixed)
+        states = (C.c_void_p * k)(*[self.local.executors[i].state.value for i in self.fixed])
+        merged = (C.c_void_p * k)(*[self.merged[i].state.value for i in self.fixed])
+        po, do, vo = ((C.c_size_t * k)(*x) for x in (parts, dims, values))
+        if self._peer is None and self._peer_ok is None:
+            self._peer = setup_peer_buffers(self.dist, sp, w, 2 * self._FLAGS_PER_PARITY + 2 * w * slot)
+            self._peer_ok = self._peer is not None
+        if self._peer is not None:
+            pe = self._peer
+            pe["epoch"] += 1
+            epoch, par = pe["epoch"], pe["epoch"] & 1   # receive buffers and flags alternate by parity
+            base, fbase = 2 * self._FLAGS_PER_PARITY + par * w * slot, par * self._FLAGS_PER_PARITY
+            slots = (C.c_void_p * w)(*[pe["ptrs"][p] + base + r * slot for p in range(w)])
+            flags = (C.c_void_p * w)(*[pe["ptrs"][p] + fbase + r * 4 for p in range(w)])
+            lib.AggStatesExportPartsToPeers(states, k, slots, flags, w, r, slot, EXCHANGE_ROWS, po, do, vo, epoch, sp.stream, sp.device)
+            lib.AggStatesMergeParts(merged, k, pe["ptrs"][r] + base, w, slot, EXCHANGE_ROWS, po, do, vo, pe["ptrs"][r] + fbase, epoch,
+                                    sp.stream, sp.device)
+            return
+        if self._send is None:
+            self._send = torch.zeros(slot, dtype=torch.uint8, device=sp.dev)
+            self._recv = torch.empty(w * slot, dtype=torch.uint8, device=sp.dev)
+        mine = (C.c_void_p * 1)(self._send.data_ptr())
+        lib.AggStatesExportPartsToPeers(states, k, mine, None, 1, 0, slot, EXCHANGE_ROWS, po, do, vo, 0, sp.stream, sp.device)
+        self.dist.all_gather_into_tensor(self._recv, self._send)
+        lib.AggStatesMergeParts(merged, k, self._recv.data_ptr(), w, slot, EXCHANGE_ROWS, po, do, vo, None, 0, sp.stream, sp.device)
+
+    def finalize(self) -> list:
+        """One result per query, in request order, identical on every rank: a QueryResult, or an HLLResult for HLL queries."""
+        if self.world == 1:
+            return self._results(self.local.executors, {})
+        if self._merged_dirty:
+            for m in self.merged:
+                m.reset()
+        self._merged_dirty = True
+        done, exact = {}, [i for i in range(len(self.queries)) if i not in self.fixed]
+        if self.fixed:
+            self._exchange_fixed()
+            for i, res in zip(self.fixed, finalize_states([self.merged[i] for i in self.fixed])):
+                if isinstance(res, A.AresError) and "exchange part truncated" in str(res):
+                    exact.append(i)
+                else:
+                    done[i] = res
+        self._keep = []
+        for i in sorted(exact):
+            rows, gathered = exchange_exact(self.dist, self.world, self.rank, self.local.executors[i], self.merged[i])
+            self._keep.append(gathered)
+            if not self.queries[i].is_hll:
+                done[i] = self.merged[i].finalize_into(rows)
+        return self._results(self.merged, done)
+
+    def _results(self, executors: list, done: dict) -> list:
+        todo = [i for i, q in enumerate(self.queries) if not q.is_hll and i not in done]
+        done.update(zip(todo, finalize_states([executors[i] for i in todo])))
+        out = []
+        for i, q in enumerate(self.queries):
+            if q.is_hll:
+                out.append(executors[i].hll_result())
+            elif isinstance(done[i], Exception):
+                raise done[i]
+            else:
+                out.append(query_result(q, *done[i]))
+        return out
+
+    def close(self):
+        self.local.close()
+        for m in self.merged or []:
+            m.close()
 
 
 # ---- host-side mirror (gloo / CPU): same protocol on QueryResults, used by the CPU test-suite ------

@@ -214,6 +214,42 @@ CGoCallResHandle AggStateMergePartsWhenFlagged(void *state, const uint8_t *parts
                                                size_t dimOffset, size_t valuesOffset, const uint32_t *flags, uint32_t epoch,
                                                void *cudaStream, int device);
 
+/* The queries of one request, several states per launch (1..16 distinct states; AGGR_HLL states are refused — they keep
+ * the exact protocol).  Every call below rejects null arrays, a numStates outside 1..16, a state given twice and an HLL
+ * state with an error.
+ *
+ * AggStatesFinalize: AggStateFinalize of states[k] into (outputKeys[k], outputValues[k]); groups[k] = its group count.
+ * States that announce at most 32768 groups are finalized by ONE launch (one cluster each) and ONE synchronise; the
+ * others, and those that turn out to need it (parked rows, more than 32768 groups), complete through AggStateFinalize's
+ * other paths within the same call, so every state gets its complete result.  When a state fails (e.g. "exchange part
+ * truncated") the others are still finalized: its groups[k] is -1 and the error lists every failed state as a line
+ * "state k: <message>".  outputKeys[k] must have states[k]'s NumDimsPerDimWidth.
+ *
+ * AggStatesExportPartsToPeers: ONE launch exports every state into its sub-part of this rank's slot — sub-part k at
+ * partOffset[k] inside the slot, laid out as AggStateExportPart's part (16-byte header [rows, status, claimed, pad],
+ * dimension block of capRows rows at dimOffset[k], measures at valuesOffset[k], both relative to the sub-part) — in
+ * peerSlots[myRank], copies every sub-part into peerSlots[r] of every peer r, and then stores `epoch` into state k's flag
+ * for this rank on every peer: peerFlags[r] + 16 * k, where peerFlags[r] = the address of flags[0][myRank] on rank r (a
+ * rank's flags are uint32 flags[state][16 ranks]).  peerFlags == NULL: the local export only (peerSlots[myRank]; the
+ * slots then travel by a collective all-gather).  capRows in [1, 32768]; slotBytes and every offset are multiples of 16,
+ * and each sub-part lies inside the slot without overlapping another; numPeers in 1..16, 0 <= myRank < numPeers.
+ *
+ * AggStatesMergeParts: ONE launch folds, for every state k, sub-part k of each of the numParts slots (slot p at
+ * slots + p * slotStride, as an all-gather or the peers' exports leave them) into states[k].  flags != NULL: the CTAs of
+ * state k first wait (bounded, as AggStateMergePartsWhenFlagged) until flags[16 * k + p] has reached `epoch` for every
+ * p < numParts; a state never waits for another state's flags.  A truncated sub-part or a late peer is reported by that
+ * state's next finalize only.  Use two flag blocks and receive buffers alternately by epoch parity, with a growing epoch.
+ * All three are asynchronous except AggStatesFinalize, which synchronises. */
+CGoCallResHandle AggStatesFinalize(void *const *states, int numStates, const DimensionVector *outputKeys, uint8_t *const *outputValues,
+                                   int64_t *groups, void *cudaStream, int device);
+CGoCallResHandle AggStatesExportPartsToPeers(void *const *states, int numStates, uint8_t *const *peerSlots, uint32_t *const *peerFlags,
+                                             int numPeers, int myRank, size_t slotBytes, int capRows, const size_t *partOffset,
+                                             const size_t *dimOffset, const size_t *valuesOffset, uint32_t epoch, void *cudaStream,
+                                             int device);
+CGoCallResHandle AggStatesMergeParts(void *const *states, int numStates, const uint8_t *slots, int numParts, size_t slotStride, int capRows,
+                                     const size_t *partOffset, const size_t *dimOffset, const size_t *valuesOffset, const uint32_t *flags,
+                                     uint32_t epoch, void *cudaStream, int device);
+
 /* AGGR_HLL states: the final outputs of the reference's last-batch HyperLogLog call
  * (query/hll.cu:262-290, adopted by query/time_series_aggregate.go:661-681).  res = number of dimension
  * groups g.  *dimValuesPtr = a DimensionVector block of VectorCapacity g (groups in key order),
