@@ -926,6 +926,7 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P, Agg
   bool measureSeen = false;
   std::vector<bool> stateFed(nmulti, false);
   P.lastFilter = -1;
+  int firstMemberFilter = -1, firstDimOrMeasure = -1;
   for (int i = 0; i < bp.NumInsts; i++) {
     const PlanInst &pi = bp.Insts[i];
     DevInst &I = P.insts[i];
@@ -983,8 +984,17 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P, Agg
         break;
       }
       case PLAN_SINK_FILTER:
+        if (firstMemberFilter >= 0) throw EngineError("member filter roots must follow the last PLAN_SINK_FILTER root");
         I.oclass = VC_BOOL;
         P.lastFilter = i;
+        break;
+      case PLAN_SINK_MEASURE_FILTER:   // (ExecuteBatchPlanMulti: a filter of state SinkArg alone)
+        if (!multi) throw EngineError("PLAN_SINK_MEASURE_FILTER (member filter) roots need ExecuteBatchPlanMulti");
+        if (pi.SinkArg >= nmulti)
+          throw EngineError("member filter root with SinkArg " + std::to_string(pi.SinkArg) + ": there are " + std::to_string(nmulti) + " states");
+        if (firstDimOrMeasure >= 0) throw EngineError("member filter roots must precede the first dimension root");
+        if (firstMemberFilter < 0) firstMemberFilter = i;
+        I.oclass = VC_BOOL;
         break;
       case PLAN_SINK_DIMENSION: {
         if (pi.SinkArg >= RL.numDims) throw EngineError("dimension ordinal outside AggSpec.NumDimsPerDimWidth");
@@ -992,6 +1002,7 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P, Agg
         if (classWidth(oc) != RL.width[pi.SinkArg]) throw EngineError("dimension data type does not match its layout width");
         if (dimSeen[pi.SinkArg]) throw EngineError("dimension written twice");
         dimSeen[pi.SinkArg] = true;
+        if (firstDimOrMeasure < 0) firstDimOrMeasure = i;
         I.oclass = oc;
         I.rowOff = RL.rowOff[pi.SinkArg];
         I.width = RL.width[pi.SinkArg];
@@ -1011,6 +1022,7 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P, Agg
           throw EngineError("only one measure per plan");
         }
         measureSeen = true;
+        if (firstDimOrMeasure < 0) firstDimOrMeasure = i;
         ValClass oc = sinkClassOf(pi.SinkDataType, false);
         if (oc != fed->measClass) throw EngineError("measure data type differs from AggSpec.MeasureDataType");
         I.oclass = oc;
@@ -1565,8 +1577,8 @@ struct MeasurePlans {
   BatchPlan &operator[](int k) { return reinterpret_cast<BatchPlan *>(mem.data())[k]; }
 };
 
-// The single-measure plan of state k: every instruction except the other states' measure roots and the sub-expressions
-// only they consume.
+// The single-measure plan of state k: every instruction except the other states' measure roots and member filter roots
+// and the sub-expressions only they consume; state k's member filters become ordinary filters.
 static void measurePlan(const BatchPlan &bp, int k, BatchPlan &out) {
   std::vector<std::vector<int>> stack;   // instructions of each stacked sub-expression
   std::vector<bool> drop(bp.NumInsts, false);
@@ -1581,7 +1593,7 @@ static void measurePlan(const BatchPlan &bp, int k, BatchPlan &out) {
     if (pi.NumOperands == 2 && pi.B.Kind == PLAN_OPERAND_STACK) pop();
     if (pi.A.Kind == PLAN_OPERAND_STACK) pop();
     if (pi.Sink == PLAN_SINK_STACK) stack.push_back(tree);
-    if (pi.Sink == PLAN_SINK_MEASURE && pi.SinkArg != k)
+    if ((pi.Sink == PLAN_SINK_MEASURE || pi.Sink == PLAN_SINK_MEASURE_FILTER) && pi.SinkArg != k)
       for (int j : tree) drop[j] = true;
   }
   memcpy(&out, &bp, sizeof(BatchPlan));
@@ -1590,6 +1602,7 @@ static void measurePlan(const BatchPlan &bp, int k, BatchPlan &out) {
     if (drop[i]) continue;
     out.Insts[n] = bp.Insts[i];
     if (out.Insts[n].Sink == PLAN_SINK_MEASURE) out.Insts[n].SinkArg = 0;
+    if (out.Insts[n].Sink == PLAN_SINK_MEASURE_FILTER) { out.Insts[n].Sink = PLAN_SINK_FILTER; out.Insts[n].SinkArg = 0; }
     n++;
   }
   out.NumInsts = n;
@@ -1633,9 +1646,26 @@ static bool planShared(AggState *const *sts, int n, const BatchPlan &bp, DevPlan
   return P.denseNd != 0;
 }
 
+// The plan one state runs for ExecuteBatchPlanMulti with numStates == 1: `bp` itself, or — when it has member filters,
+// checked as in a shared plan — `bp` with them turned into filters (stored in `one`).
+static const BatchPlan &singleStatePlan(AggState *const *sts, const BatchPlan &bp, MeasurePlans &one) {
+  bool memberFilters = false;
+  for (int i = 0; i < bp.NumInsts && i < ARES_MAX_PLAN_INSTS; i++) memberFilters = memberFilters || bp.Insts[i].Sink == PLAN_SINK_MEASURE_FILTER;
+  if (!memberFilters) return bp;
+  static thread_local DevPlan Q;
+  compilePlan(sts[0], bp, Q, sts, 1);
+  one.resize(1);
+  measurePlan(bp, 0, one[0]);
+  return one[0];
+}
+
 static void executePlanMulti(AggState *const *sts, int n, const BatchPlan &bp, cudaStream_t s) {
   checkSharedStates(sts, n);
-  if (n == 1) { executePlan(sts[0], bp, s); return; }
+  if (n == 1) {
+    MeasurePlans one;
+    executePlan(sts[0], singleStatePlan(sts, bp, one), s);
+    return;
+  }
   if (bp.NumRows > 0x7FFFFFFFu) throw EngineError("a batch holds at most 2^31-1 rows");
   static thread_local DevPlan P;
   MeasurePlans subs;
@@ -2355,8 +2385,9 @@ CGoCallResHandle AresJitDryRunMulti(const AggSpec *specs, int numSpecs, const Ba
     static thread_local DevPlan P;
     MeasurePlans subs;
     if (numSpecs == 1) {
-      compilePlan(sts[0], *plan, P);
-      prepareInputs(P, *plan, nullptr, nullptr);
+      const BatchPlan &one = singleStatePlan(sts, *plan, subs);
+      compilePlan(sts[0], one, P);
+      prepareInputs(P, one, nullptr, nullptr);
       layoutStages(P, specs[0].ExpectedGroups);
     } else if (!planShared(sts, numSpecs, *plan, P, subs, nullptr, nullptr)) {
       throw EngineError("this plan and zone map run one kernel per state (no shared direct-indexed form)");

@@ -7,6 +7,11 @@
 #ifndef JIT_NMEAS
 #define JIT_NMEAS 1
 #endif
+// Plans with member filters (PLAN_SINK_MEASURE_FILTER) define JIT_LIVE_ARG(x) as `, x`: their evaluators then report in
+// live[M] the rows alive for measure M.  Without, every measure takes every alive row (live[M] stays 0xF).
+#ifndef JIT_LIVE_ARG
+#define JIT_LIVE_ARG(x)
+#endif
 namespace aresb {
 
 __device__ __forceinline__ void jitIssueTile(const JitParams &P, uint32_t tile, uint8_t *stage, uint64_t *bar) {
@@ -297,19 +302,27 @@ static __device__ __noinline__ void multiColdRows(const uint8_t *stage, uint32_t
                                                   uint32_t inRange, uint32_t s0, uint32_t s1, uint32_t s2, uint32_t s3) {
   uint64_t key[4][JIT_KW], mv[JIT_NMEAS][4];
   const uint32_t slot[4] = {s0, s1, s2, s3};
-  uint32_t alive = rowEvalGeneric(stage, q, row0, P, key, mv[0] JIT_MEAS_REST1(mv));
+  uint32_t live[JIT_NMEAS];
+#pragma unroll
+  for (int m = 0; m < JIT_NMEAS; m++) live[m] = 0xFu;
+  uint32_t alive = rowEvalGeneric(stage, q, row0, P, key, mv[0] JIT_MEAS_REST1(mv) JIT_LIVE_ARG(live));
   alive &= (1u << nvalid) - 1u;
-#define JIT_STEP(M) multiColdMeasure<M>(P, alive, inRange, key, mv[M], slot);
+  // (a cold row claims a group only in the tables of the measures it is alive for)
+#define JIT_STEP(M) multiColdMeasure<M>(P, alive & live[M], inRange, key, mv[M], slot);
   JIT_EACH_MEASURE(JIT_STEP)
 #undef JIT_STEP
 }
 
+// `live`: the rows of the quad alive for measure M (bit r); `fast` holds the rows alive for some measure inside the zone map
 template <int M>
-__device__ __forceinline__ bool multiDenseMeasure(uint32_t tableAddr, const JitParams &P, const bool (&fast)[4], const uint32_t (&s)[4],
-                                                  const uint64_t (&meas)[4], const uint32_t (&mraw)[4]) {
+__device__ __forceinline__ bool multiDenseMeasure(uint32_t tableAddr, const JitParams &P, const bool (&fastAny)[4], uint32_t live,
+                                                  const uint32_t (&s)[4], const uint64_t (&meas)[4], const uint32_t (&mraw)[4]) {
   constexpr int OP = kMeasOp[M];
   const uint32_t base = tableAddr + kMeasSmemOff[M];
   bool cold = false;
+  bool fast[4];
+#pragma unroll
+  for (int r = 0; r < 4; r++) fast[r] = fastAny[r] && ((live >> r) & 1u) != 0;
   if (kMeasAcc[M] == 4) {
 #pragma unroll
     for (int r = 0; r < 4; r++) {
@@ -350,11 +363,11 @@ __device__ __forceinline__ bool multiDenseMeasure(uint32_t tableAddr, const JitP
 __device__ __forceinline__ void multiAggregateDense(uint32_t tableAddr, const JitParams &P, const uint8_t *stage, uint32_t q, uint32_t row0,
                                                     uint32_t nvalid, uint32_t repOff, const bool (&fast)[4], bool cold,
                                                     const uint32_t (&dslot)[4], const uint64_t (&mv)[JIT_NMEAS][4],
-                                                    const uint32_t (&mr)[JIT_NMEAS][4]) {
+                                                    const uint32_t (&mr)[JIT_NMEAS][4], const uint32_t (&live)[JIT_NMEAS]) {
   uint32_t s[4];
 #pragma unroll
   for (int r = 0; r < 4; r++) s[r] = dslot[r] + repOff;
-#define JIT_STEP(M) cold = multiDenseMeasure<M>(tableAddr, P, fast, s, mv[M], mr[M]) || cold;
+#define JIT_STEP(M) cold = multiDenseMeasure<M>(tableAddr, P, fast, live[M], s, mv[M], mr[M]) || cold;
   JIT_EACH_MEASURE(JIT_STEP)
 #undef JIT_STEP
   if (cold) {
@@ -598,9 +611,11 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
         uint32_t dslot[4];
         bool fast[4], anySlow;
         uint64_t mv[JIT_NMEAS][4];
-        uint32_t mr[JIT_NMEAS][4];
-        if (rowEval(stage, q, t * JIT_TILE_ROWS + q * 4, P, 4u, fast, anySlow, dslot, mv[0], mr[0] JIT_MEAS_REST(mv, mr)))
-          multiAggregateDense(touchedAddr, P, stage, q, t * JIT_TILE_ROWS + q * 4, 4u, repOff, fast, anySlow, dslot, mv, mr);
+        uint32_t mr[JIT_NMEAS][4], live[JIT_NMEAS];
+#pragma unroll
+        for (int m = 0; m < JIT_NMEAS; m++) live[m] = 0xFu;
+        if (rowEval(stage, q, t * JIT_TILE_ROWS + q * 4, P, 4u, fast, anySlow, dslot, mv[0], mr[0] JIT_MEAS_REST(mv, mr) JIT_LIVE_ARG(live)))
+          multiAggregateDense(touchedAddr, P, stage, q, t * JIT_TILE_ROWS + q * 4, 4u, repOff, fast, anySlow, dslot, mv, mr, live);
         (void)meas; (void)allowClaim; (void)bypass;
 #elif JIT_DENSE
         uint32_t dslot[4];
@@ -658,9 +673,11 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
         uint32_t dslot[4];
         bool fast[4], anySlow;
         uint64_t mv[JIT_NMEAS][4];
-        uint32_t mr[JIT_NMEAS][4];
-        if (rowEval(stages, q, done + q * 4, P, nvalid, fast, anySlow, dslot, mv[0], mr[0] JIT_MEAS_REST(mv, mr)))
-          multiAggregateDense(touchedAddr, P, stages, q, done + q * 4, nvalid, repOff, fast, anySlow, dslot, mv, mr);
+        uint32_t mr[JIT_NMEAS][4], live[JIT_NMEAS];
+#pragma unroll
+        for (int m = 0; m < JIT_NMEAS; m++) live[m] = 0xFu;
+        if (rowEval(stages, q, done + q * 4, P, nvalid, fast, anySlow, dslot, mv[0], mr[0] JIT_MEAS_REST(mv, mr) JIT_LIVE_ARG(live)))
+          multiAggregateDense(touchedAddr, P, stages, q, done + q * 4, nvalid, repOff, fast, anySlow, dslot, mv, mr, live);
         (void)meas;
 #elif JIT_DENSE
         uint32_t dslot[4];

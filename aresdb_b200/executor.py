@@ -7,8 +7,8 @@
   engine, or (in tests / the CPU baseline) a HOST-mode build running on host memory.
 * `FusedBatchExecutor` is the B200-native form: one ExecuteBatchPlan call per batch into a
   device-resident AggState, one AggStateFinalize per query.
-* `FusedRequestExecutor` runs the queries of one AQL request: queries that share filters, dimensions and joins read each
-  batch once (ExecuteBatchPlanMulti, one state per query).
+* `FusedRequestExecutor` runs the queries of one AQL request: queries that share dimensions, time filter and joins read
+  each batch once (ExecuteBatchPlanMulti, one state per query; filters they do not all have are member filters).
 
 Both take batches as lists of `VectorPartySlice`s that already live in the executor's memory space.
 """
@@ -540,15 +540,17 @@ def _finalize_some(exs: list) -> list:
 MAX_SHARED_MEASURES = 4   # measure roots (states) of one ExecuteBatchPlanMulti plan
 
 
-def shared_scan_groups(queries: list) -> list[list[int]]:
+def shared_scan_groups(queries: list, member_filters: bool = False) -> list[list[int]]:
     """Indexes of `queries` grouped for one pass: queries with the same plan instructions except the measure root (same
     filters in the same order, time-filter range, dimensions), the same joins and reduce mode, and no HLL; at most
-    MAX_SHARED_MEASURES per group, in request order.  Every other query is a group of its own."""
+    MAX_SHARED_MEASURES per group, in request order.  Every other query is a group of its own.
+    `member_filters`: queries whose filters differ group as well (same dimensions, time filter, joins and reduce mode);
+    a query whose filters would make the group's plan longer than ARES_MAX_PLAN_INSTS starts a new group."""
     groups, open_group = [], {}
     for i, q in enumerate(queries):
-        key = q.shared_scan_key()
+        key = q.shared_scan_key(member_filters=member_filters)
         g = open_group.get(key) if key is not None else None
-        if g is None or len(g) >= MAX_SHARED_MEASURES:
+        if g is None or len(g) >= MAX_SHARED_MEASURES or (member_filters and not _plan_fits([queries[j] for j in g + [i]])):
             g = []
             groups.append(g)
             if key is not None:
@@ -557,40 +559,65 @@ def shared_scan_groups(queries: list) -> list[list[int]]:
     return groups
 
 
+def _plan_fits(members: list) -> bool:
+    """The shared plan of `members` (with the cutoff filter of a live batch, its longest variant) stays within the plan
+    limits."""
+    lead = members[0]
+    try:
+        lead.plan_instructions(cutoff=1, measures=members)
+    except ValueError:
+        return False
+    return len(lead.foreign_columns) <= A.ARES_MAX_FOREIGN_COLUMNS
+
+
 class FusedRequestExecutor:
     """The queries of one AQL request (aql.compile_request): each keeps its own AggState and result, and the queries of a
-    compatible group (shared_scan_groups) read every batch once — one ExecuteBatchPlanMulti call whose plan carries one
-    measure root per query.  The engine picks the form per batch: one kernel for all of them, or each query's own kernel."""
+    compatible group (shared_scan_groups with member filters: same dimensions, time filter, joins and reduce mode) read
+    every batch once — one ExecuteBatchPlanMulti call whose plan carries the filters they all have, each query's own
+    filters as member filters, and one measure root per query.  The engine picks the form per batch: one kernel for all of
+    them, or each query's own kernel."""
 
     def __init__(self, lib: A.Library, space, queries: list, expected_groups: int | list = 0):
         """`expected_groups`: one hint for every query, or a list with one per query."""
         self.lib, self.space, self.queries = lib, space, list(queries)
         eg = list(expected_groups) if isinstance(expected_groups, (list, tuple)) else [expected_groups] * len(self.queries)
         self.executors = [FusedBatchExecutor(lib, space, q, g) for q, g in zip(self.queries, eg)]
-        self.groups = shared_scan_groups(self.queries)
-        self._shared = {}
-        for g in self.groups:
-            if len(g) > 1:
-                lead, members = self.queries[g[0]], [self.queries[i] for i in g]
-                self._shared[g[0]] = _BatchPlans(lead, lambda tf, co, lead=lead, members=members:
-                                                 lead.plan_instructions(time_filters=tf, cutoff=co, measures=members))
+        self.groups = shared_scan_groups(self.queries, member_filters=True)
+        self._shared = {}   # (indexes of the queries that run a batch together) -> their _BatchPlans
         self.calls = 0
 
+    def _plans(self, members: tuple) -> _BatchPlans:
+        """The plans of the members of a group that run a batch: the whole group, or the members whose filters the
+        batch's zone map does not contradict (built on first use, like the time-filter variants)."""
+        p = self._shared.get(members)
+        if p is None:
+            lead, qs = self.queries[members[0]], [self.queries[i] for i in members]
+            p = self._shared[members] = _BatchPlans(lead, lambda tf, co: lead.plan_instructions(time_filters=tf, cutoff=co,
+                                                                                               measures=qs))
+        return p
+
     def process_batch(self, batch: Batch, stream=None, time_filters: bool = True, cutoff: int = 0):
-        """Same meaning as FusedBatchExecutor.process_batch, for every query of the request."""
+        """Same meaning as FusedBatchExecutor.process_batch, for every query of the request.  A query whose filters the
+        batch's zone map contradicts skips the batch as it would alone; the other queries of its group run it together."""
         for g in self.groups:
-            ex = self.executors[g[0]]
             if len(g) == 1:
-                ex.process_batch(batch, stream, time_filters, cutoff)
+                self.executors[g[0]].process_batch(batch, stream, time_filters, cutoff)
                 continue
-            if should_skip_batch(ex.q, batch.ranges):   # (the group's filters are the same)
-                for i in g:
+            run = []
+            for i in g:
+                if should_skip_batch(self.queries[i], batch.ranges):
                     self.executors[i].skipped += 1
+                else:
+                    run.append(i)
+            if not run:
                 continue
-            p = self._shared[g[0]].plan_for(batch, time_filters, cutoff)
-            states = (C.c_void_p * len(g))(*[self.executors[i].state.value for i in g])
+            if len(run) == 1:
+                self.executors[run[0]].process_batch(batch, stream, time_filters, cutoff)
+                continue
+            p = self._plans(tuple(run)).plan_for(batch, time_filters, cutoff)
+            states = (C.c_void_p * len(run))(*[self.executors[i].state.value for i in run])
             self.calls += 1
-            self.lib.ExecuteBatchPlanMulti(states, len(g), C.byref(p), self.space.stream if stream is None else stream,
+            self.lib.ExecuteBatchPlanMulti(states, len(run), C.byref(p), self.space.stream if stream is None else stream,
                                            self.space.device)
 
     def results(self) -> list:

@@ -129,8 +129,11 @@ class AggQuery:
         """Post-order flattening of every expression: one PlanInst per non-leaf AST node (what
         processExpression turns into one cgo call, reference query/time_series_aggregate.go:493-593).
         `time_filters=False`: the plan of an archive batch strictly inside the query's time range.
-        `measures`: queries sharing this query's filters and dimensions (shared_scan_key); the plan ends with their
-        measure roots, root k (SinkArg k) feeding the k-th state of ExecuteBatchPlanMulti."""
+        `measures`: queries sharing this query's dimensions, time filter, joins and reduce mode (shared_scan_key); the
+        plan ends with their measure roots, root k (SinkArg k) feeding the k-th state of ExecuteBatchPlanMulti.  The
+        filters every one of them carries come first, in this query's order; each query's other filters follow as member
+        filter roots (PLAN_SINK_MEASURE_FILTER, SinkArg k), before the dimensions."""
+        members = [self] if measures is None else measures
         insts: list[A.PlanInst] = []
         self.foreign_columns = []   # distinct (table, column, timezone) leaves in first-use order = BatchPlan.ForeignColumns
 
@@ -167,31 +170,44 @@ class AggQuery:
             pi.Sink, pi.SinkArg, pi.SinkDataType = sink, sink_arg, sink_dt
             insts.append(pi)
 
+        # (structural comparison: the instruction bytes of a foreign column depend on the plan it is in)
+        common = [all(any(f == g for g in m.filters) for m in members) for f in self.filters]
         lo, hi = self.time_filter_range
         for i, f in enumerate(self.filters):
             if i == lo and cutoff > 0:          # the custom-filter step: cutoff filter first, then the time filters
                 emit(self.cutoff_filter(cutoff), A.PLAN_SINK_FILTER, 0, A.Bool)
-            if time_filters or not lo <= i < hi:
+            if common[i] and (time_filters or not lo <= i < hi):
                 emit(f, A.PLAN_SINK_FILTER, 0, A.Bool)
         if cutoff > 0 and lo >= len(self.filters):
             emit(self.cutoff_filter(cutoff), A.PLAN_SINK_FILTER, 0, A.Bool)
+        shared = [f for f, c in zip(self.filters, common) if c]
+        for k, q in enumerate(members):
+            for f in q.filters:
+                if not any(f == g for g in shared):
+                    emit(f, A.PLAN_SINK_MEASURE_FILTER, k, A.Bool)
         for pos, qi in enumerate(self.dim_order):
             emit(self.dimensions[qi], A.PLAN_SINK_DIMENSION, pos, self.dim_types[qi])
-        for k, q in enumerate([self] if measures is None else measures):
+        for k, q in enumerate(members):
             emit(q.measure, A.PLAN_SINK_MEASURE, k, q.measure_data_type)
         if len(insts) > A.ARES_MAX_PLAN_INSTS:
             raise ValueError("plan too long")
         return insts
 
 
-    def shared_scan_key(self):
+    def shared_scan_key(self, member_filters: bool = False):
         """What queries must agree on to read the batches in one pass: the plan up to the measure root (filters in order,
         with their literals, and dimensions), the time-filter positions, the joins and the reduce mode.  None for HLL
-        queries, which never share."""
+        queries, which never share.  `member_filters`: the filters may differ (each query's own filters become member
+        filters of the shared plan); the dimensions, the time filter, the joins and the reduce mode must not."""
         if self.is_hll:
             return None
-        prefix = tuple(bytes(pi) for pi in self.plan_instructions(measures=[]))
         joins = tuple((id(j.table), j.on.index, j.timezone_ptr, j.timezone_size) for j in self.joins)
+        if member_filters:
+            lo, hi = self.time_filter_range
+            # (expressions compare structurally: their repr is the key)
+            dims = repr([(self.dimensions[qi], self.dim_types[qi]) for qi in self.dim_order])
+            return dims, repr(self.filters[lo:hi]), joins, self.reduce_mode
+        prefix = tuple(bytes(pi) for pi in self.plan_instructions(measures=[]))
         return prefix, self.time_filter_range, joins, self.reduce_mode
 
 

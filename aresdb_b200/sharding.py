@@ -231,7 +231,7 @@ def request_slot_layout(queries: list, cap_rows: int = EXCHANGE_ROWS):
 
 class ShardedFusedRequest:
     """One rank's half of a sharded AQL request (torch.distributed / NCCL plumbing).  The rank's batches are scanned by a
-    FusedRequestExecutor, so queries that share filters and dimensions share the scan on every rank.  finalize() exchanges
+    FusedRequestExecutor, so queries that share dimensions, time filter and joins share the scan on every rank.  finalize() exchanges
     every non-HLL query that announces at most EXCHANGE_ROWS groups in ONE export launch (the rank's slot holds one
     sub-part per query; over peer memory when every rank can map every other's receive buffer, else one NCCL all-gather
     — ARESDB_B200_EXCHANGE as for ShardedFusedQuery), folds them with ONE merge launch and finalizes them with ONE

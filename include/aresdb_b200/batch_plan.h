@@ -57,15 +57,18 @@ enum PlanSink {
   PLAN_SINK_STACK = 0,     /* non-root node: ScratchSpaceOutput of DataType SinkDataType       */
   PLAN_SINK_FILTER = 1,    /* root of a filter: row survives iff bool(value) (filterAction)      */
   PLAN_SINK_DIMENSION = 2, /* root of dimension #SinkArg (layout order), DimensionOutput         */
-  PLAN_SINK_MEASURE = 3    /* root of the measure, MeasureOutput of SinkDataType / AggSpec.AggFunc; ExecuteBatchPlanMulti:
+  PLAN_SINK_MEASURE = 3,   /* root of the measure, MeasureOutput of SinkDataType / AggSpec.AggFunc; ExecuteBatchPlanMulti:
                             * one root per state, SinkArg = the ordinal of the state it feeds */
+  PLAN_SINK_MEASURE_FILTER = 4 /* ExecuteBatchPlanMulti only: root of a filter that applies to state SinkArg alone (a
+                                * member filter, see ExecuteBatchPlanMulti) */
 };
 
 typedef struct {
   uint8_t NumOperands;  /* 1: Functor is a UnaryFunctorType; 2: a BinaryFunctorType */
   uint8_t Functor;
   uint8_t Sink;         /* enum PlanSink */
-  uint8_t SinkArg;      /* dimension ordinal for PLAN_SINK_DIMENSION; state ordinal for PLAN_SINK_MEASURE (Multi) */
+  uint8_t SinkArg;      /* dimension ordinal for PLAN_SINK_DIMENSION; state ordinal for PLAN_SINK_MEASURE and
+                         * PLAN_SINK_MEASURE_FILTER (Multi) */
   uint8_t SinkDataType; /* enum DataType of the sink element */
   uint8_t Reserved[3];
   PlanOperand A;
@@ -163,7 +166,17 @@ CGoCallResHandle ExecuteBatchPlan(void *state, const BatchPlan *plan, void *cuda
  * ReduceMode, and none may be AGGR_HLL.  When the batch's zone map lets every measure's own single-measure plan take the
  * CTA's direct-indexed slots and they all fit a CTA together, one kernel evaluates each row once and feeds every state;
  * otherwise each state runs its single-measure plan (what ExecuteBatchPlan would launch).  Results are the same either
- * way.  numStates == 1 is ExecuteBatchPlan.  Asynchronous like ExecuteBatchPlan. */
+ * way.  numStates == 1 is ExecuteBatchPlan.  Asynchronous like ExecuteBatchPlan.
+ *
+ * Member filters: the states may also differ in their filters.  A PLAN_SINK_MEASURE_FILTER root applies to state
+ * SinkArg only; a row feeds state k iff it passes every PLAN_SINK_FILTER root and every PLAN_SINK_MEASURE_FILTER root
+ * with SinkArg == k.  Filters every state carries are PLAN_SINK_FILTER roots and are evaluated once per row.  Member
+ * filter roots follow the last PLAN_SINK_FILTER root and precede the first PLAN_SINK_DIMENSION root.  Rejected with an
+ * error string: a member filter in a plan given to ExecuteBatchPlan, a SinkArg outside 0..numStates-1, and member
+ * filter roots out of that order.  In the one-kernel form a row's dimensions are computed when it is alive for some
+ * state, and each state's accumulators see only the rows alive for it; in the per-state form state k runs its
+ * single-measure plan, which keeps state k's member filters as ordinary filters and drops the other states' member
+ * filters.  numStates == 1 is ExecuteBatchPlan of the plan with its member filters turned into filters. */
 CGoCallResHandle ExecuteBatchPlanMulti(void *const *states, int numStates, const BatchPlan *plan, void *cudaStream, int device);
 
 /* Folds already-reduced rows (a DimensionVector block + measure vector, e.g. the carried

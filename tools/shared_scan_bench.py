@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""The cfg3 table (8 day-batches x 1.25e8 rows, zone maps) queried by one dashboard request: {sum(fare), count(*)} and
-a four-measure request {sum(fare), count(*), avg(fare), max(city_id)}, each run in one pass (FusedRequestExecutor) and
-as separate queries (one FusedBatchExecutor each), alternating in the same process.  Times are CUDA events around the
-batches of a step plus the finalize of every query; the results of both forms are compared before anything is timed.
+"""The cfg3 table (8 day-batches x 1.25e8 rows, zone maps) queried by one dashboard request: {sum(fare), count(*)},
+a four-measure request {sum(fare), count(*), avg(fare), max(city_id)}, and a request whose queries differ in their filters
+(common part: the time range and city_id != 0; members: sum(fare) where status = 1 and fare > 5, count(*) where
+status = 1, count(*) where status = 2, count(*)), each run in one pass (FusedRequestExecutor) and as separate queries (one
+FusedBatchExecutor each), alternating in the same process.  Times are CUDA events around the batches of a step plus the finalize of every query; the results of both forms are compared before anything is timed.
 Usage: python tools/shared_scan_bench.py [--steps N] [--batches B] [--rows R]"""
 import argparse
 import json
@@ -24,7 +25,7 @@ def main():
     import torch
     import bench
     from aresdb_b200 import cabi as A, columns, expr as E, synth
-    from aresdb_b200.executor import Batch, FusedBatchExecutor, FusedRequestExecutor
+    from aresdb_b200.executor import Batch, FusedBatchExecutor, FusedRequestExecutor, shared_scan_groups
     from aresdb_b200.memory import CudaSpace
     from aresdb_b200.query import AggQuery, Measure
 
@@ -35,8 +36,11 @@ def main():
     dims = base.dimensions
     ms = [Measure("sum", E.Col(3, A.Float32, "fare")), Measure("count"), Measure("avg", E.Col(3, A.Float32, "fare")),
           Measure("max", E.Col(1, A.Uint16, "city_id"))]
+    status1, status2, rest = base.filters[0], E.eq(bench._columns()[2], E.Lit(2)), base.filters[2:]
     requests = {"sum_count": [AggQuery(base.filters, dims, m) for m in ms[:2]],
-                "four_measures": [AggQuery(base.filters, dims, m) for m in ms]}
+                "four_measures": [AggQuery(base.filters, dims, m) for m in ms],
+                "differing_filters": [AggQuery(base.filters, dims, ms[0]), AggQuery([status1] + rest, dims, ms[1]),
+                                      AggQuery([status2] + rest, dims, ms[1]), AggQuery(rest, dims, ms[1])]}
     keep, batches = [], []
     for d in range(args.batches):
         bufs, voff = synth.generate_batch_cuda(d, args.rows, dev)
@@ -99,7 +103,8 @@ def main():
             t["shared"] += timed("shared", qs)
             t["separate"] += timed("separate", qs)
         med = {k: float(np.median(v)) for k, v in t.items()}
-        report["requests"][name] = {"measures": len(qs), "shared_ms": med["shared"], "separate_ms": med["separate"],
+        report["requests"][name] = {"measures": len(qs), "groups": shared_scan_groups(qs, member_filters=True),
+                                    "shared_ms": med["shared"], "separate_ms": med["separate"],
                                     "shared_ms_all": t["shared"], "separate_ms_all": t["separate"],
                                     "speedup": med["separate"] / med["shared"], "results_equal": True}
         print(f"{name}: one pass {med['shared']:.2f} ms, separate queries {med['separate']:.2f} ms "
