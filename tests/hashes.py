@@ -14,10 +14,10 @@ def _rotl32(x, r):
 
 
 def murmur3_32(rows: np.ndarray) -> np.ndarray:
-    """rows: uint8[n, len] with len a multiple of 4 -> uint32[n] (seed 0)."""
+    """rows: uint8[n, len] -> uint32[n] (seed 0)."""
     n, ln = rows.shape
-    assert ln % 4 == 0
-    words = np.ascontiguousarray(rows).view("<u4").reshape(n, ln // 4).astype(np.uint64)
+    rows = np.ascontiguousarray(rows)
+    words = np.ascontiguousarray(rows[:, :ln // 4 * 4]).view("<u4").reshape(n, ln // 4).astype(np.uint64)
     h = np.zeros(n, np.uint64)
     for i in range(ln // 4):
         k = (words[:, i] * np.uint64(0xcc9e2d51)) & M32
@@ -26,6 +26,14 @@ def murmur3_32(rows: np.ndarray) -> np.ndarray:
         h ^= k
         h = _rotl32(h, 13)
         h = (h * np.uint64(5) + np.uint64(0xe6546b64)) & M32
+    if ln % 4:   # the 1-3 tail bytes, little-endian, without the block's final rotate-multiply-add
+        k = np.zeros(n, np.uint64)
+        for j in range(ln % 4):
+            k |= rows[:, ln // 4 * 4 + j].astype(np.uint64) << np.uint64(8 * j)
+        k = (k * np.uint64(0xcc9e2d51)) & M32
+        k = _rotl32(k, 15)
+        k = (k * np.uint64(0x1b873593)) & M32
+        h ^= k
     h ^= np.uint64(ln)
     h ^= h >> np.uint64(16)
     h = (h * np.uint64(0x85ebca6b)) & M32
