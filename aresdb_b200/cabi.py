@@ -49,7 +49,7 @@ VectorPartyInput, ScratchSpaceInput, ConstantInput, ForeignColumnInput, ArrayVec
 ScratchSpaceOutput, MeasureOutput, DimensionOutput = range(3)
 
 PLAN_OPERAND_NONE, PLAN_OPERAND_COLUMN, PLAN_OPERAND_CONST, PLAN_OPERAND_STACK, PLAN_OPERAND_FOREIGN = range(5)
-PLAN_SINK_STACK, PLAN_SINK_FILTER, PLAN_SINK_DIMENSION, PLAN_SINK_MEASURE, PLAN_SINK_MEASURE_FILTER = range(5)
+PLAN_SINK_STACK, PLAN_SINK_FILTER, PLAN_SINK_DIMENSION, PLAN_SINK_MEASURE, PLAN_SINK_MEASURE_FILTER, PLAN_SINK_MEMBER_DIMENSION = range(6)
 ARES_REDUCE_SORT, ARES_REDUCE_HASH = range(2)
 ARES_MAX_PLAN_COLUMNS = 32
 ARES_MAX_PLAN_INSTS = 64

@@ -926,7 +926,9 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P, Agg
   bool measureSeen = false;
   std::vector<bool> stateFed(nmulti, false);
   P.lastFilter = -1;
-  int firstMemberFilter = -1, firstDimOrMeasure = -1;
+  int firstMemberFilter = -1, firstDimOrMeasure = -1, firstMeasure = -1;
+  bool plainDims = false;
+  std::vector<int> memberDimsOf(nmulti, 0);   // member dimension roots of each state so far
   for (int i = 0; i < bp.NumInsts; i++) {
     const PlanInst &pi = bp.Insts[i];
     DevInst &I = P.insts[i];
@@ -956,8 +958,10 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P, Agg
     if (wideIn) {
       // only "dimension = 8/16-byte column" is meaningful (what UnaryTransform Noop to a
       // DimensionOutput of the same type does)
-      ValClass oc = pi.Sink == PLAN_SINK_DIMENSION ? sinkClassOf(pi.SinkDataType, true) : VC_NONE;
-      if (pi.NumOperands != 1 || pi.Functor != Noop || pi.Sink != PLAN_SINK_DIMENSION || pi.A.Kind != PLAN_OPERAND_COLUMN ||
+      // (a wide member dimension never reaches the kernel as one: the direct-indexed form the member form needs has none)
+      const bool dimSink = pi.Sink == PLAN_SINK_DIMENSION || pi.Sink == PLAN_SINK_MEMBER_DIMENSION;
+      ValClass oc = dimSink ? sinkClassOf(pi.SinkDataType, true) : VC_NONE;
+      if (pi.NumOperands != 1 || pi.Functor != Noop || !dimSink || pi.A.Kind != PLAN_OPERAND_COLUMN ||
           oc != (ValClass)acls)
         throw EngineError("int64/UUID columns are only supported as verbatim dimensions on the fused path");
       I.wide = 1;
@@ -996,7 +1000,36 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P, Agg
         if (firstMemberFilter < 0) firstMemberFilter = i;
         I.oclass = VC_BOOL;
         break;
+      case PLAN_SINK_MEMBER_DIMENSION: {   // (ExecuteBatchPlanMulti: a dimension of the states in mask SinkArg)
+        if (!multi) throw EngineError("PLAN_SINK_MEMBER_DIMENSION (member dimension) roots need ExecuteBatchPlanMulti");
+        if (pi.SinkArg == 0) throw EngineError("member dimension root with an empty state mask");
+        if (pi.SinkArg >> nmulti)
+          throw EngineError("member dimension root with state mask " + std::to_string(pi.SinkArg) + ": there are " + std::to_string(nmulti) + " states");
+        if (plainDims) throw EngineError("a plan has PLAN_SINK_DIMENSION or PLAN_SINK_MEMBER_DIMENSION roots, not both");
+        if (firstMeasure >= 0) throw EngineError("member dimension roots must precede the measure roots");
+        if (firstDimOrMeasure < 0) firstDimOrMeasure = i;
+        const ValClass oc = sinkClassOf(pi.SinkDataType, true);
+        const int u = P.memberDims++;   // this root is member dimension u (dense dimension u of the shared form)
+        if (u >= kJitMaxDenseDims * kJitMaxMeasures) throw EngineError("too many member dimension roots");
+        for (int k = 0; k < nmulti; k++) {
+          if (!((pi.SinkArg >> k) & 1)) continue;
+          const DimLayout &L = multi[k]->rowLayout;
+          const int j = memberDimsOf[k]++;
+          if (j >= L.numDims || classWidth(oc) != L.width[j])
+            throw EngineError("member dimension roots of state " + std::to_string(k) + " do not match its NumDimsPerDimWidth");
+          if (u < kJitMaxDenseDims) {
+            P.meas[k].dims |= (uint8_t)(1u << u);
+            P.meas[k].rowOff[u] = L.rowOff[j];
+            P.meas[k].nullOff[u] = (uint8_t)(L.valueBytes + j);
+          }
+        }
+        I.oclass = oc;
+        I.width = (uint8_t)classWidth(oc);
+        break;
+      }
       case PLAN_SINK_DIMENSION: {
+        if (P.memberDims) throw EngineError("a plan has PLAN_SINK_DIMENSION or PLAN_SINK_MEMBER_DIMENSION roots, not both");
+        plainDims = true;
         if (pi.SinkArg >= RL.numDims) throw EngineError("dimension ordinal outside AggSpec.NumDimsPerDimWidth");
         ValClass oc = sinkClassOf(pi.SinkDataType, true);
         if (classWidth(oc) != RL.width[pi.SinkArg]) throw EngineError("dimension data type does not match its layout width");
@@ -1023,6 +1056,7 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P, Agg
         }
         measureSeen = true;
         if (firstDimOrMeasure < 0) firstDimOrMeasure = i;
+        if (firstMeasure < 0) firstMeasure = i;
         ValClass oc = sinkClassOf(pi.SinkDataType, false);
         if (oc != fed->measClass) throw EngineError("measure data type differs from AggSpec.MeasureDataType");
         I.oclass = oc;
@@ -1032,8 +1066,11 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P, Agg
     }
   }
   if (!stack.empty()) throw EngineError("plan leaves values on the evaluation stack");
-  for (int d = 0; d < RL.numDims; d++)
+  for (int d = 0; d < RL.numDims && !P.memberDims; d++)
     if (!dimSeen[d]) throw EngineError("plan does not produce every dimension of AggSpec");
+  for (int k = 0; k < nmulti && P.memberDims; k++)
+    if (memberDimsOf[k] != multi[k]->rowLayout.numDims)
+      throw EngineError("member dimension roots of state " + std::to_string(k) + " do not match its NumDimsPerDimWidth");
   if (!measureSeen) throw EngineError("plan has no measure instruction");
   for (int k = 0; k < nmulti; k++)
     if (!stateFed[k]) throw EngineError("no measure root feeds state " + std::to_string(k) + " (missing SinkArg)");
@@ -1129,6 +1166,31 @@ static bool stagesBaseCounts(const DevPlan &P) {
 // Decides the tile size, the stage layout, the TMA ring depth and the shared table size.  The shared table gets what the
 // workload needs first (a table that overflows sends rows to contended L2 atomics, tools/microbench/agg_microbench.cu),
 // the ring takes the rest.  Staged parts must start on a 16-byte boundary (executePlan copies those that do not).
+// Member dimensions: the slots of each measure's region when `avail` bytes of shared memory hold them, false when they do
+// not.  Each region holds at least the measure's own slots; the rest of `avail` is shared in proportion to them (for
+// lane-private copies of few slots).
+static bool memberSlots(DevPlan &P, size_t avail) {
+  size_t need = 0, sb[kJitMaxMeasures], r16[kJitMaxMeasures];
+  for (int m = 0; m < P.nmeas; m++) {
+    DevMeasure &M = P.meas[m];
+    uint64_t total = 1;
+    for (int j = 0; j < P.denseNd && total <= kDenseMaxSlots; j++)
+      if ((M.dims >> j) & 1u) total *= (uint64_t)P.denseCnt[j] + 1;
+    if (total > kDenseMaxSlots) return false;
+    M.total = (uint32_t)total;
+    sb[m] = M.denseFx ? 12 : 9;
+    r16[m] = (total + 15) / 16 * 16;
+    need += r16[m] * sb[m];
+  }
+  if (avail < 128u * P.nmeas + need) return false;
+  avail -= 128u * P.nmeas;   // (each region starts on a 128-byte boundary)
+  for (int m = 0; m < P.nmeas; m++) {
+    const size_t cap = r16[m] * avail / need / 16 * 16;
+    P.meas[m].slots = (uint32_t)(cap < kDenseMaxSlots ? cap : kDenseMaxSlots);
+  }
+  return true;
+}
+
 static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
   const bool stageBc = stagesBaseCounts(P);
   // The shared table takes 8192 slots (128 KB) whenever a ring of >= 2 stages still fits beside
@@ -1167,8 +1229,15 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
     for (uint32_t tr : {3968u, 1920u, 896u}) {
       for (uint32_t n = kMaxStages; n >= 2 && !tileRows; n--) {
         // (several measures: one 128-byte aligned region of accumulators each)
-        const size_t need = 128 + n * stageBytesFor(tr) + (P.nmeas > 1 ? 128 * P.nmeas : 0);
+        const size_t need = 128 + n * stageBytesFor(tr) + (P.nmeas > 1 && !P.memberDims ? 128 * P.nmeas : 0);
         if (need >= (size_t)kSmemBudget) continue;
+        if (P.memberDims) {   // (only with several measures: planShared)
+          if (memberSlots(P, (size_t)kSmemBudget - need)) {
+            tileRows = tr; stages = n; slots = 16;
+            for (int m = 0; m < P.nmeas; m++) slots = P.meas[m].slots > slots ? P.meas[m].slots : slots;
+          }
+          continue;
+        }
         // three 32-bit piece counters, or flag + 8-byte accumulator; HLL: one 32-bit map entry (slot -> group's registers)
         size_t slotBytes = P.hll ? 4 : P.denseFx ? 12 : 9;
         if (P.nmeas > 1) {
@@ -1244,7 +1313,8 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
   P.tableBytes = P.denseNd != 0 ? (slots * (P.hll ? 4 : P.denseFx ? 12 : 9) + 127) / 128 * 128 : slots * 8;
   if (P.nmeas > 1) {
     P.tableBytes = 0;
-    for (int m = 0; m < P.nmeas; m++) P.tableBytes += (slots * (P.meas[m].denseFx ? 12 : 9) + 127) / 128 * 128;
+    for (int m = 0; m < P.nmeas; m++)
+      P.tableBytes += ((P.memberDims ? P.meas[m].slots : slots) * (P.meas[m].denseFx ? 12 : 9) + 127) / 128 * 128;
   }
   return 128 + (size_t)P.tableBytes + stageBytes * P.numStages;
 }
@@ -1559,12 +1629,20 @@ static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
 // ---------------------------------------------------------------------------------------
 // several measures over one scan (ExecuteBatchPlanMulti)
 // ---------------------------------------------------------------------------------------
-// States that may share a plan: the same dimension layout and reduce mode, no HLL.
-static void checkSharedStates(AggState *const *sts, int n) {
+static bool hasSink(const BatchPlan &bp, int sink) {
+  for (int i = 0; i < bp.NumInsts && i < ARES_MAX_PLAN_INSTS; i++)
+    if (bp.Insts[i].Sink == sink) return true;
+  return false;
+}
+
+// States that may share a plan: the same reduce mode, no HLL, and the same dimension layout unless the plan gives each
+// state its own dimensions (member dimensions, checked by compilePlan).
+static void checkSharedStates(AggState *const *sts, int n, const BatchPlan &bp) {
   if (n < 1 || n > kJitMaxMeasures) throw EngineError("numStates must be 1.." + std::to_string(kJitMaxMeasures));
+  const bool memberDims = hasSink(bp, PLAN_SINK_MEMBER_DIMENSION);
   for (int k = 0; k < n; k++) {
     if (sts[k]->hll) throw EngineError("AGGR_HLL states cannot share a plan");
-    if (memcmp(sts[k]->spec.NumDimsPerDimWidth, sts[0]->spec.NumDimsPerDimWidth, NUM_DIM_WIDTH) != 0)
+    if (!memberDims && memcmp(sts[k]->spec.NumDimsPerDimWidth, sts[0]->spec.NumDimsPerDimWidth, NUM_DIM_WIDTH) != 0)
       throw EngineError("states differ in NumDimsPerDimWidth");
     if (sts[k]->spec.ReduceMode != sts[0]->spec.ReduceMode) throw EngineError("states differ in ReduceMode");
   }
@@ -1577,9 +1655,11 @@ struct MeasurePlans {
   BatchPlan &operator[](int k) { return reinterpret_cast<BatchPlan *>(mem.data())[k]; }
 };
 
-// The single-measure plan of state k: every instruction except the other states' measure roots and member filter roots
-// and the sub-expressions only they consume; state k's member filters become ordinary filters.
-static void measurePlan(const BatchPlan &bp, int k, BatchPlan &out) {
+// The plan of the states in `set` (bit k = state k): every instruction except the other states' measure, member filter
+// and member dimension roots and the sub-expressions only they consume.  The kept states are renumbered in order; their
+// member dimensions become PLAN_SINK_DIMENSION roots (ordinals in plan order: the states of a set have the same
+// dimensions), and the member filters of a single state become ordinary filters.
+static void measurePlan(const BatchPlan &bp, uint32_t set, BatchPlan &out) {
   std::vector<std::vector<int>> stack;   // instructions of each stacked sub-expression
   std::vector<bool> drop(bp.NumInsts, false);
   for (int i = 0; i < bp.NumInsts; i++) {
@@ -1593,30 +1673,56 @@ static void measurePlan(const BatchPlan &bp, int k, BatchPlan &out) {
     if (pi.NumOperands == 2 && pi.B.Kind == PLAN_OPERAND_STACK) pop();
     if (pi.A.Kind == PLAN_OPERAND_STACK) pop();
     if (pi.Sink == PLAN_SINK_STACK) stack.push_back(tree);
-    if ((pi.Sink == PLAN_SINK_MEASURE || pi.Sink == PLAN_SINK_MEASURE_FILTER) && pi.SinkArg != k)
+    const bool other = ((pi.Sink == PLAN_SINK_MEASURE || pi.Sink == PLAN_SINK_MEASURE_FILTER) && !((set >> pi.SinkArg) & 1u)) ||
+                       (pi.Sink == PLAN_SINK_MEMBER_DIMENSION && (pi.SinkArg & set) == 0);
+    if (other)
       for (int j : tree) drop[j] = true;
   }
+  const bool single = (set & (set - 1)) == 0;
+  auto rank = [&](int k) { return (uint8_t)__builtin_popcount(set & ((1u << k) - 1u)); };
   memcpy(&out, &bp, sizeof(BatchPlan));
-  int n = 0;
+  int n = 0, dims = 0;
   for (int i = 0; i < bp.NumInsts; i++) {
     if (drop[i]) continue;
-    out.Insts[n] = bp.Insts[i];
-    if (out.Insts[n].Sink == PLAN_SINK_MEASURE) out.Insts[n].SinkArg = 0;
-    if (out.Insts[n].Sink == PLAN_SINK_MEASURE_FILTER) { out.Insts[n].Sink = PLAN_SINK_FILTER; out.Insts[n].SinkArg = 0; }
-    n++;
+    PlanInst &pi = out.Insts[n++];
+    pi = bp.Insts[i];
+    if (pi.Sink == PLAN_SINK_MEASURE) pi.SinkArg = rank(pi.SinkArg);
+    if (pi.Sink == PLAN_SINK_MEASURE_FILTER) {
+      if (single) pi.Sink = PLAN_SINK_FILTER;
+      pi.SinkArg = single ? 0 : rank(pi.SinkArg);
+    }
+    if (pi.Sink == PLAN_SINK_MEMBER_DIMENSION) { pi.Sink = PLAN_SINK_DIMENSION; pi.SinkArg = (uint8_t)dims++; }
   }
   out.NumInsts = n;
 }
 
+// The states of a plan with member dimensions grouped by their dimensions: one mask (bit k = state k) per distinct set
+// of member dimension roots, in the order of each set's first state.
+static std::vector<uint32_t> dimensionSets(int n, const BatchPlan &bp) {
+  std::vector<std::vector<bool>> sig(n, std::vector<bool>(bp.NumInsts, false));
+  for (int i = 0; i < bp.NumInsts; i++)
+    for (int k = 0; k < n; k++)
+      sig[k][i] = bp.Insts[i].Sink == PLAN_SINK_MEMBER_DIMENSION && ((bp.Insts[i].SinkArg >> k) & 1u);
+  std::vector<uint32_t> sets;
+  std::vector<int> lead;
+  for (int k = 0; k < n; k++) {
+    size_t j = 0;
+    while (j < lead.size() && sig[lead[j]] != sig[k]) j++;
+    if (j == lead.size()) { lead.push_back(k); sets.push_back(0); }
+    sets[j] |= 1u << k;
+  }
+  return sets;
+}
+
 // Compiles the shared plan into P and decides its form for this batch.  true: one kernel feeds every state — each
 // measure's own single-measure plan takes the CTA's direct-indexed slots, and all of them fit a CTA together (P is then
-// laid out, without device work when `scratch` is null).  false: the caller runs subs[k] on state k, one kernel each.
-// `subs` is filled either way.
+// laid out, without device work when `scratch` is null).  false: the caller runs the states' own plans, or (member
+// dimensions) the plans of the states' dimension sets.  `subs` holds the single-measure plans either way.
 static bool planShared(AggState *const *sts, int n, const BatchPlan &bp, DevPlan &P, MeasurePlans &subs,
                        cudaStream_t s, std::vector<std::unique_ptr<Scratch>> *scratch) {
   compilePlan(sts[0], bp, P, sts, n);
   subs.resize(n);
-  for (int k = 0; k < n; k++) measurePlan(bp, k, subs[k]);
+  for (int k = 0; k < n; k++) measurePlan(bp, 1u << k, subs[k]);
   if (bp.NumRows == 0) return false;
   static thread_local DevPlan Q;
   bool shared = true;
@@ -1630,6 +1736,10 @@ static bool planShared(AggState *const *sts, int n, const BatchPlan &bp, DevPlan
     M.aggOp = Q.aggOp; M.measWidth = Q.measWidth; M.skipCount = Q.skipCount; M.neutralSafe = Q.neutralSafe;
     M.denseFx = Q.denseFx; M.fxShift = Q.fxShift; M.measureIdentity = Q.measureIdentity; M.accNeutral = Q.accNeutral;
     skipCount = skipCount && Q.skipCount;
+    // member dimensions: every state packs its rows with the kernel's one key form (JIT_KW / JIT_ROW_BYTES)
+    if (P.memberDims && (sts[k]->keyMode != sts[0]->keyMode ||
+                         (sts[k]->keyMode == KEY_HASHED && sts[k]->rowLayout.rowBytes != sts[0]->rowLayout.rowBytes)))
+      shared = false;
   }
   if (!shared) return false;
   P.nmeas = (uint8_t)n;
@@ -1646,21 +1756,28 @@ static bool planShared(AggState *const *sts, int n, const BatchPlan &bp, DevPlan
   return P.denseNd != 0;
 }
 
-// The plan one state runs for ExecuteBatchPlanMulti with numStates == 1: `bp` itself, or — when it has member filters,
-// checked as in a shared plan — `bp` with them turned into filters (stored in `one`).
+// The plan one state runs for ExecuteBatchPlanMulti with numStates == 1: `bp` itself, or — when it has member filters
+// or member dimensions, checked as in a shared plan — `bp` with them turned into filters and dimensions (stored in `one`).
 static const BatchPlan &singleStatePlan(AggState *const *sts, const BatchPlan &bp, MeasurePlans &one) {
-  bool memberFilters = false;
-  for (int i = 0; i < bp.NumInsts && i < ARES_MAX_PLAN_INSTS; i++) memberFilters = memberFilters || bp.Insts[i].Sink == PLAN_SINK_MEASURE_FILTER;
-  if (!memberFilters) return bp;
+  if (!hasSink(bp, PLAN_SINK_MEASURE_FILTER) && !hasSink(bp, PLAN_SINK_MEMBER_DIMENSION)) return bp;
   static thread_local DevPlan Q;
   compilePlan(sts[0], bp, Q, sts, 1);
   one.resize(1);
-  measurePlan(bp, 0, one[0]);
+  measurePlan(bp, 1u, one[0]);
   return one[0];
 }
 
+// The states of `set` and the plan of their dimension set (member dimensions become their dimensions).
+static int setStates(AggState *const *sts, uint32_t set, const BatchPlan &bp, AggState **out, BatchPlan &plan) {
+  int m = 0;
+  for (int k = 0; k < kJitMaxMeasures; k++)
+    if ((set >> k) & 1u) out[m++] = sts[k];
+  measurePlan(bp, set, plan);
+  return m;
+}
+
 static void executePlanMulti(AggState *const *sts, int n, const BatchPlan &bp, cudaStream_t s) {
-  checkSharedStates(sts, n);
+  checkSharedStates(sts, n, bp);
   if (n == 1) {
     MeasurePlans one;
     executePlan(sts[0], singleStatePlan(sts, bp, one), s);
@@ -1671,6 +1788,17 @@ static void executePlanMulti(AggState *const *sts, int n, const BatchPlan &bp, c
   MeasurePlans subs;
   std::vector<std::unique_ptr<Scratch>> scratch;
   if (!planShared(sts, n, bp, P, subs, s, &scratch)) {
+    if (P.memberDims) {   // one pass per dimension set, each deciding its own form (never more kernels than states)
+      const std::vector<uint32_t> sets = dimensionSets(n, bp);
+      MeasurePlans plans;
+      plans.resize((int)sets.size());
+      for (size_t j = 0; j < sets.size(); j++) {
+        AggState *ss[kJitMaxMeasures];
+        const int m = setStates(sts, sets[j], bp, ss, plans[(int)j]);
+        executePlanMulti(ss, m, plans[(int)j], s);
+      }
+      return;
+    }
     for (int k = 0; k < n; k++) executePlan(sts[k], subs[k], s);
     return;
   }
@@ -1681,7 +1809,7 @@ static void executePlanMulti(AggState *const *sts, int n, const BatchPlan &bp, c
   rleTileHints(P, bp, s, scratch);
   // direct-indexed kernels are not waited for: every state gets room for what the flush may insert up front
   for (int k = 0; k < n; k++) {
-    ensureRoom(sts[k], (uint64_t)P.denseTotal, s);
+    ensureRoom(sts[k], (uint64_t)(P.memberDims ? P.meas[k].total : P.denseTotal), s);
     P.meas[k].G = sts[k]->table;
     P.meas[k].ctaAcc = sts[k]->ctaAcc;
   }
@@ -2381,7 +2509,7 @@ CGoCallResHandle AresJitDryRunMulti(const AggSpec *specs, int numSpecs, const Ba
       st[k].capacity = 0;
       sts[k] = &st[k];
     }
-    checkSharedStates(sts, numSpecs);
+    checkSharedStates(sts, numSpecs, *plan);
     static thread_local DevPlan P;
     MeasurePlans subs;
     if (numSpecs == 1) {
@@ -2390,6 +2518,28 @@ CGoCallResHandle AresJitDryRunMulti(const AggSpec *specs, int numSpecs, const Ba
       prepareInputs(P, one, nullptr, nullptr);
       layoutStages(P, specs[0].ExpectedGroups);
     } else if (!planShared(sts, numSpecs, *plan, P, subs, nullptr, nullptr)) {
+      if (P.memberDims) {   // the per-set form: does every dimension set run as one direct-indexed kernel?
+        const std::vector<uint32_t> sets = dimensionSets(numSpecs, *plan);
+        std::unique_ptr<DevPlan> Q(new DevPlan);
+        MeasurePlans plans, more;
+        plans.resize((int)sets.size());
+        bool direct = true;
+        for (size_t j = 0; j < sets.size() && direct; j++) {
+          AggState *ss[kJitMaxMeasures];
+          const int m = setStates(sts, sets[j], *plan, ss, plans[(int)j]);
+          if (m > 1) {
+            direct = planShared(ss, m, plans[(int)j], *Q, more, nullptr, nullptr);
+          } else {
+            compilePlan(ss[0], plans[(int)j], *Q);
+            prepareInputs(*Q, plans[(int)j], nullptr, nullptr);
+            layoutStages(*Q, ss[0]->spec.ExpectedGroups);
+            direct = Q->denseNd != 0;
+          }
+        }
+        if (direct)
+          throw EngineError("this plan and zone map run one kernel per dimension set (" + std::to_string(sets.size()) +
+                            " sets, each direct-indexed)");
+      }
       throw EngineError("this plan and zone map run one kernel per state (no shared direct-indexed form)");
     }
     std::string src;

@@ -12,6 +12,22 @@
 #ifndef JIT_LIVE_ARG
 #define JIT_LIVE_ARG(x)
 #endif
+// Plans whose measures differ in their dimensions (PLAN_SINK_MEMBER_DIMENSION) define JIT_MDIMS 1 and the per-measure
+// tables kMeasCap (slots of the measure's region) and kMeasDims (its dimensions, bit k = dense dimension k): rowEval then
+// gives each measure its own slot (dslot[M]), rowEvalGeneric the dimension values instead of a packed key, and
+// memberPack<M> packs measure M's row.
+#ifndef JIT_MDIMS
+#define JIT_MDIMS 0
+#endif
+#if JIT_MDIMS
+#define JIT_NSLOT JIT_NMEAS
+#define JIT_DSLOT(d) d
+#define JIT_DIM_ARG(dv, dvb) , dv, dvb
+#else
+#define JIT_NSLOT 1
+#define JIT_DSLOT(d) d[0]
+#define JIT_DIM_ARG(dv, dvb)
+#endif
 namespace aresb {
 
 __device__ __forceinline__ void jitIssueTile(const JitParams &P, uint32_t tile, uint8_t *stage, uint64_t *bar) {
@@ -273,6 +289,29 @@ __device__ __forceinline__ void jitAggregateDense(uint32_t touchedAddr, unsigned
 #define JIT_EACH_MEASURE(STEP) { STEP(0) STEP(1) if (JIT_NMEAS > 2) { STEP((JIT_NMEAS > 2 ? 2 : 0)) } if (JIT_NMEAS > 3) { STEP((JIT_NMEAS > 3 ? 3 : 0)) } }
 template <int M>
 __device__ __forceinline__ unsigned long long *measSlice(const JitParams &P) { return P.ms[M].ctaAcc + (size_t)blockIdx.x * JIT_SMEM_SLOTS; }
+// slots of measure M's region, its dimensions, and the slots its CTA-private copies span
+template <int M>
+__device__ __forceinline__ uint32_t measCap() {
+#if JIT_MDIMS
+  return kMeasCap[M];
+#else
+  return kDenseCap;
+#endif
+}
+template <int M>
+__device__ __forceinline__ uint32_t measDims() {
+#if JIT_MDIMS
+  return kMeasDims[M];
+#else
+  return 0xFFu;
+#endif
+}
+template <int M>
+__device__ __forceinline__ uint32_t measSlots(const JitParams &P, uint32_t denseSlots) {
+  return JIT_MDIMS ? P.mRepStride[M] * P.mReps[M] : denseSlots;
+}
+// a quad's slots: one set (shared dimensions) or one per measure (JIT_MDIMS)
+struct JitSlots { uint32_t v[JIT_NSLOT][4]; };
 
 template <int M>
 __device__ __forceinline__ void multiColdMeasure(const JitParams &P, uint32_t alive, uint32_t inRange, const uint64_t (&key)[4][JIT_KW],
@@ -299,16 +338,25 @@ __device__ __forceinline__ void multiColdMeasure(const JitParams &P, uint32_t al
 
 // the rows some measure's fast path could not finish, evaluated again with full generality (out of line, rare)
 static __device__ __noinline__ void multiColdRows(const uint8_t *stage, uint32_t q, uint32_t row0, const JitParams &P, uint32_t nvalid,
-                                                  uint32_t inRange, uint32_t s0, uint32_t s1, uint32_t s2, uint32_t s3) {
+                                                  uint32_t inRange, const JitSlots s) {
   uint64_t key[4][JIT_KW], mv[JIT_NMEAS][4];
-  const uint32_t slot[4] = {s0, s1, s2, s3};
   uint32_t live[JIT_NMEAS];
 #pragma unroll
   for (int m = 0; m < JIT_NMEAS; m++) live[m] = 0xFu;
-  uint32_t alive = rowEvalGeneric(stage, q, row0, P, key, mv[0] JIT_MEAS_REST1(mv) JIT_LIVE_ARG(live));
+#if JIT_MDIMS
+  uint32_t dv[4][JIT_ND], dvb[4];
+#endif
+  uint32_t alive = rowEvalGeneric(stage, q, row0, P, key, mv[0] JIT_MEAS_REST1(mv) JIT_DIM_ARG(dv, dvb) JIT_LIVE_ARG(live));
   alive &= (1u << nvalid) - 1u;
-  // (a cold row claims a group only in the tables of the measures it is alive for)
-#define JIT_STEP(M) multiColdMeasure<M>(P, alive & live[M], inRange, key, mv[M], slot);
+  // (a cold row claims a group only in the tables of the measures it is alive for, keyed by their own dimensions)
+#if JIT_MDIMS
+#define JIT_STEP(M) {                                                  \
+    uint64_t mkey[4][JIT_KW];                                          \
+    _Pragma("unroll") for (int r = 0; r < 4; r++) memberPack<M>(dv[r], dvb[r], mkey[r]); \
+    multiColdMeasure<M>(P, alive & live[M], inRange, mkey, mv[M], s.v[JIT_MDIMS ? M : 0]); }
+#else
+#define JIT_STEP(M) multiColdMeasure<M>(P, alive & live[M], inRange, key, mv[M], s.v[0]);
+#endif
   JIT_EACH_MEASURE(JIT_STEP)
 #undef JIT_STEP
 }
@@ -349,11 +397,11 @@ __device__ __forceinline__ bool multiDenseMeasure(uint32_t tableAddr, const JitP
       for (int r = 0; r < 4; r++) stsFlag(base + s[r], go[r]);
     }
     unsigned long long *tAcc = measSlice<M>(P);
-    unsigned long long *generic = reinterpret_cast<unsigned long long *>(denseSmemBase() + kMeasSmemOff[M] + kDenseCap);
+    unsigned long long *generic = reinterpret_cast<unsigned long long *>(denseSmemBase() + kMeasSmemOff[M] + measCap<M>());
     constexpr int kToShared = kMeasAcc[M] == 1 ? 4 : 2;
 #pragma unroll
     for (int r = 0; r < 4; r++) {
-      if (r < kToShared) redSharedPred<OP>(base + kDenseCap + 8u * s[r], generic + s[r], meas[r], go[r]);
+      if (r < kToShared) redSharedPred<OP>(base + measCap<M>() + 8u * s[r], generic + s[r], meas[r], go[r]);
       else redGlobalPred<OP>(tAcc + s[r], meas[r], go[r]);
     }
   }
@@ -362,17 +410,22 @@ __device__ __forceinline__ bool multiDenseMeasure(uint32_t tableAddr, const JitP
 
 __device__ __forceinline__ void multiAggregateDense(uint32_t tableAddr, const JitParams &P, const uint8_t *stage, uint32_t q, uint32_t row0,
                                                     uint32_t nvalid, uint32_t repOff, const bool (&fast)[4], bool cold,
-                                                    const uint32_t (&dslot)[4], const uint64_t (&mv)[JIT_NMEAS][4],
+                                                    const uint32_t (&dslot)[JIT_NSLOT][4], const uint64_t (&mv)[JIT_NMEAS][4],
                                                     const uint32_t (&mr)[JIT_NMEAS][4], const uint32_t (&live)[JIT_NMEAS]) {
-  uint32_t s[4];
+  // (JIT_MDIMS: each measure's lane-private copy follows its own slot count)
+  JitSlots s;
 #pragma unroll
-  for (int r = 0; r < 4; r++) s[r] = dslot[r] + repOff;
-#define JIT_STEP(M) cold = multiDenseMeasure<M>(tableAddr, P, fast, live[M], s, mv[M], mr[M]) || cold;
+  for (int m = 0; m < JIT_NSLOT; m++) {
+    const uint32_t off = JIT_MDIMS ? (threadIdx.x & (P.mReps[m] - 1u)) * P.mRepStride[m] : repOff;
+#pragma unroll
+    for (int r = 0; r < 4; r++) s.v[m][r] = dslot[m][r] + off;
+  }
+#define JIT_STEP(M) cold = multiDenseMeasure<M>(tableAddr, P, fast, live[M], s.v[JIT_MDIMS ? M : 0], mv[M], mr[M]) || cold;
   JIT_EACH_MEASURE(JIT_STEP)
 #undef JIT_STEP
   if (cold) {
     const uint32_t inRange = (fast[0] ? 1u : 0u) | (fast[1] ? 2u : 0u) | (fast[2] ? 4u : 0u) | (fast[3] ? 8u : 0u);
-    multiColdRows(stage, q, row0, P, nvalid, inRange, s[0], s[1], s[2], s[3]);
+    multiColdRows(stage, q, row0, P, nvalid, inRange, s);
   }
 }
 
@@ -381,14 +434,15 @@ __device__ __forceinline__ void multiInitMeasure(const JitParams &P, uint32_t de
   {
     uint8_t *base = denseSmemBase() + kMeasSmemOff[M];
     unsigned long long *tAcc = measSlice<M>(P);
-    for (uint32_t i = threadIdx.x; i < denseSlots; i += JIT_THREADS) {
+    const uint32_t n = measSlots<M>(P, denseSlots);
+    for (uint32_t i = threadIdx.x; i < n; i += JIT_THREADS) {
       if (kMeasAcc[M] != 1) tAcc[i] = P.ms[M].accNeutral;
       if (kMeasAcc[M] == 4) {
         uint32_t *c = reinterpret_cast<uint32_t *>(base) + 3u * i;
         c[0] = 0; c[1] = 0; c[2] = 0;
       } else {
         if (kMeasFlags[M]) base[i] = 0;
-        reinterpret_cast<unsigned long long *>(base + kDenseCap)[i] = P.ms[M].accNeutral;
+        reinterpret_cast<unsigned long long *>(base + measCap<M>())[i] = P.ms[M].accNeutral;
       }
     }
   }
@@ -407,28 +461,37 @@ __device__ __forceinline__ void multiFlushMeasure(const JitParams &P, uint32_t d
     const uint8_t *base = denseSmemBase() + kMeasSmemOff[M];
     unsigned long long *tAcc = measSlice<M>(P);
     const unsigned long long neutral = P.ms[M].accNeutral;
-    for (uint32_t i = threadIdx.x; i < denseSlots; i += JIT_THREADS) {
+    const uint32_t n = measSlots<M>(P, denseSlots);
+    for (uint32_t i = threadIdx.x; i < n; i += JIT_THREADS) {
       unsigned long long accS = neutral;
       if (kMeasAcc[M] == 4) {
         const uint32_t *c = reinterpret_cast<const uint32_t *>(base) + 3u * i;
         const unsigned long long v = (unsigned long long)c[0] + ((unsigned long long)c[1] << 11) + ((unsigned long long)c[2] << 22);
         if (v != 0) accS = (unsigned long long)__double_as_longlong(__ull2double_rn(v) * P.ms[M].fxInv);
       } else {
-        accS = reinterpret_cast<const unsigned long long *>(base + kDenseCap)[i];
+        accS = reinterpret_cast<const unsigned long long *>(base + measCap<M>())[i];
       }
       const unsigned long long accG = kMeasAcc[M] != 1 ? __ldcg(&tAcc[i]) : neutral;
       if (kMeasFlags[M] ? !base[i] : (accS == neutral && accG == neutral)) continue;
-      uint32_t rem = i % P.dRepStride, dvr[JIT_ND], vb = 0;
+      // (JIT_MDIMS: measure M's slot decodes over its own dimensions and strides)
+      uint32_t rem = i % (JIT_MDIMS ? P.mRepStride[M] : P.dRepStride), dvr[JIT_ND], vb = 0;
 #pragma unroll
       for (int k = JIT_ND - 1; k >= 0; k--) {
-        const uint32_t ix = rem / P.dStride[k];
-        rem -= ix * P.dStride[k];
+        dvr[k] = 0u;
+        if (!((measDims<M>() >> k) & 1u)) continue;
+        const uint32_t stride = JIT_MDIMS ? P.mStride[M][k] : P.dStride[k];
+        const uint32_t ix = rem / stride;
+        rem -= ix * stride;
         const bool valid = ix != P.dCnt[k];
         dvr[k] = valid ? (P.dLo[k] + ix) * P.dStep[k] : 0u;
         vb |= (valid ? 1u : 0u) << k;
       }
       uint64_t key[JIT_KW];
+#if JIT_MDIMS
+      memberPack<M>(dvr, vb, key);
+#else
       densePack(dvr, vb, key);
+#endif
       const unsigned long long k = jitKeyOfRow(key);
       if (kMeasAcc[M] != 1) globalUpdate<M>(P.ms[M].G, (AggOp)OP, k, JIT_KW == 1 ? nullptr : key, accG, true);
       globalUpdate<M>(P.ms[M].G, (AggOp)OP, k, JIT_KW == 1 ? nullptr : key, accS, true);
@@ -608,13 +671,13 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
         const uint32_t q = threadIdx.x;
         uint64_t meas[4];
 #if JIT_DENSE && JIT_NMEAS > 1
-        uint32_t dslot[4];
+        uint32_t dslot[JIT_NSLOT][4];
         bool fast[4], anySlow;
         uint64_t mv[JIT_NMEAS][4];
         uint32_t mr[JIT_NMEAS][4], live[JIT_NMEAS];
 #pragma unroll
         for (int m = 0; m < JIT_NMEAS; m++) live[m] = 0xFu;
-        if (rowEval(stage, q, t * JIT_TILE_ROWS + q * 4, P, 4u, fast, anySlow, dslot, mv[0], mr[0] JIT_MEAS_REST(mv, mr) JIT_LIVE_ARG(live)))
+        if (rowEval(stage, q, t * JIT_TILE_ROWS + q * 4, P, 4u, fast, anySlow, JIT_DSLOT(dslot), mv[0], mr[0] JIT_MEAS_REST(mv, mr) JIT_LIVE_ARG(live)))
           multiAggregateDense(touchedAddr, P, stage, q, t * JIT_TILE_ROWS + q * 4, 4u, repOff, fast, anySlow, dslot, mv, mr, live);
         (void)meas; (void)allowClaim; (void)bypass;
 #elif JIT_DENSE
@@ -670,13 +733,13 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
         uint64_t meas[4];
         const uint32_t nvalid = rows - q * 4 < 4 ? rows - q * 4 : 4;
 #if JIT_DENSE && JIT_NMEAS > 1
-        uint32_t dslot[4];
+        uint32_t dslot[JIT_NSLOT][4];
         bool fast[4], anySlow;
         uint64_t mv[JIT_NMEAS][4];
         uint32_t mr[JIT_NMEAS][4], live[JIT_NMEAS];
 #pragma unroll
         for (int m = 0; m < JIT_NMEAS; m++) live[m] = 0xFu;
-        if (rowEval(stages, q, done + q * 4, P, nvalid, fast, anySlow, dslot, mv[0], mr[0] JIT_MEAS_REST(mv, mr) JIT_LIVE_ARG(live)))
+        if (rowEval(stages, q, done + q * 4, P, nvalid, fast, anySlow, JIT_DSLOT(dslot), mv[0], mr[0] JIT_MEAS_REST(mv, mr) JIT_LIVE_ARG(live)))
           multiAggregateDense(touchedAddr, P, stages, q, done + q * 4, nvalid, repOff, fast, anySlow, dslot, mv, mr, live);
         (void)meas;
 #elif JIT_DENSE

@@ -73,6 +73,10 @@ struct JitParams {
   uint32_t startCount;                    // row number of index position 0 when the batch has no base counts
   RleColumn rle[kJitMaxRle];              // run-length encoded columns decoded in place (see ldrle)
   JitMeasure ms[kJitMaxMeasures];         // JIT_NMEAS > 1: measure m's state (unused by single-measure kernels)
+  // JIT_MDIMS (the measures differ in their dimensions): measure m's slot = sum_k index_k * mStride[m][k] (0 for a
+  // dimension m does not have); lane-private copies of its slots, mRepStride[m] slots apart
+  uint32_t mStride[kJitMaxMeasures][kJitMaxDenseDims];
+  uint32_t mReps[kJitMaxMeasures], mRepStride[kJitMaxMeasures];
 };
 // (with every measure's group table in it: the block stays far below the 32 KB kernel-parameter limit of sm_90)
 static_assert(sizeof(JitParams) <= 4096, "the kernel's parameter block is limited to 4 KB");

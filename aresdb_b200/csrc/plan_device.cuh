@@ -55,6 +55,12 @@ struct DevMeasure {
   int8_t inst;                   // the measure root in the shared plan
   int8_t fxShift;
   uint8_t aggOp, measWidth, skipCount, neutralSafe, denseFx, pad;
+  // member dimensions (DevPlan::memberDims): the state's dimensions among the plan's (bit j = dense dimension j), where
+  // each sits in the state's row (byte offset of the value, of the validity byte; by member dimension root), its slots
+  // (prod of (count + 1) over its dimensions) and the slots of its region in the CTA (>= total, set by layoutStages)
+  uint8_t dims;
+  uint8_t rowOff[kJitMaxDenseDims], nullOff[kJitMaxDenseDims];
+  uint32_t total, slots;
 };
 
 struct DevPlan {
@@ -106,6 +112,7 @@ struct DevPlan {
   const DevJoin *join;     // device copy of the tables' indexes and the foreign columns' batches
   uint32_t resume;         // 1: relaunch of the same batch after the group table grew (DevTable::progress holds the resume points)
   uint8_t nmeas;           // > 1: measure roots feeding that many states (direct-indexed form only); meas[] describes them
+  uint8_t memberDims;      // PLAN_SINK_MEMBER_DIMENSION roots of the plan (0: plain dimension roots; the states differ in theirs)
   DevMeasure meas[kJitMaxMeasures];
 };
 

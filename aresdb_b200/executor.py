@@ -23,7 +23,7 @@ import numpy as np
 from . import cabi as A
 from . import expr as E
 from .memory import Buf
-from .query import AggQuery, HLLResult, QueryResult
+from .query import AggQuery, HLLResult, QueryResult, member_dimensions
 from .skipping import should_skip_batch
 
 
@@ -559,6 +559,41 @@ def shared_scan_groups(queries: list, member_filters: bool = False) -> list[list
     return groups
 
 
+MAX_PASS_DIMENSIONS = 8   # union dimensions of one pass: what the kernel indexes directly (kJitMaxDenseDims)
+
+
+def shared_scan_passes(queries: list, groups: list) -> list[list[int]]:
+    """`groups` (shared_scan_groups with member filters) packed into passes over the batches: groups that agree in time
+    filter, joins and reduce mode, with dimensions and without HLL, share a pass (their dimensions become member
+    dimensions of its plan) while it has at most MAX_SHARED_MEASURES queries and MAX_PASS_DIMENSIONS dimensions, its plan
+    fits the plan limits, and its queries order their dimensions consistently (query.member_dimensions).  Returns the
+    indexes of each pass's queries, group by group, in request order."""
+    passes, open_pass = [], {}
+    for g in groups:
+        q = queries[g[0]]
+        key = q.shared_scan_key(member_filters=True)
+        key = key[1:] if key is not None and q.dimensions else None
+        p = open_pass.get(key) if key is not None else None
+        if p is not None and _pass_fits([queries[i] for i in p + g]):
+            p.extend(g)
+            continue
+        p = list(g)
+        passes.append(p)
+        if key is not None:
+            open_pass[key] = p
+    return passes
+
+
+def _pass_fits(members: list) -> bool:
+    if len(members) > MAX_SHARED_MEASURES:
+        return False
+    try:
+        union = member_dimensions(members)
+    except ValueError:
+        return False
+    return (union is None or len(union) <= MAX_PASS_DIMENSIONS) and _plan_fits(members)
+
+
 def _plan_fits(members: list) -> bool:
     """The shared plan of `members` (with the cutoff filter of a live batch, its longest variant) stays within the plan
     limits."""
@@ -571,11 +606,13 @@ def _plan_fits(members: list) -> bool:
 
 
 class FusedRequestExecutor:
-    """The queries of one AQL request (aql.compile_request): each keeps its own AggState and result, and the queries of a
-    compatible group (shared_scan_groups with member filters: same dimensions, time filter, joins and reduce mode) read
-    every batch once — one ExecuteBatchPlanMulti call whose plan carries the filters they all have, each query's own
-    filters as member filters, and one measure root per query.  The engine picks the form per batch: one kernel for all of
-    them, or each query's own kernel."""
+    """The queries of one AQL request (aql.compile_request): each keeps its own AggState and result.  `groups` are the
+    compatible groups (shared_scan_groups with member filters: same dimensions, time filter, joins and reduce mode);
+    `passes` packs groups that differ only in their dimensions (shared_scan_passes).  The queries of a pass read every
+    batch once — one ExecuteBatchPlanMulti call whose plan carries the filters they all have, each query's own filters as
+    member filters, their dimensions (as member dimensions when they differ), and one measure root per query.  The engine
+    picks the form per batch: one kernel for all of them, one kernel per set of queries with the same dimensions, or each
+    query's own kernel."""
 
     def __init__(self, lib: A.Library, space, queries: list, expected_groups: int | list = 0):
         """`expected_groups`: one hint for every query, or a list with one per query."""
@@ -583,11 +620,12 @@ class FusedRequestExecutor:
         eg = list(expected_groups) if isinstance(expected_groups, (list, tuple)) else [expected_groups] * len(self.queries)
         self.executors = [FusedBatchExecutor(lib, space, q, g) for q, g in zip(self.queries, eg)]
         self.groups = shared_scan_groups(self.queries, member_filters=True)
+        self.passes = shared_scan_passes(self.queries, self.groups)
         self._shared = {}   # (indexes of the queries that run a batch together) -> their _BatchPlans
         self.calls = 0
 
     def _plans(self, members: tuple) -> _BatchPlans:
-        """The plans of the members of a group that run a batch: the whole group, or the members whose filters the
+        """The plans of the members of a pass that run a batch: the whole pass, or the members whose filters the
         batch's zone map does not contradict (built on first use, like the time-filter variants)."""
         p = self._shared.get(members)
         if p is None:
@@ -598,8 +636,8 @@ class FusedRequestExecutor:
 
     def process_batch(self, batch: Batch, stream=None, time_filters: bool = True, cutoff: int = 0):
         """Same meaning as FusedBatchExecutor.process_batch, for every query of the request.  A query whose filters the
-        batch's zone map contradicts skips the batch as it would alone; the other queries of its group run it together."""
-        for g in self.groups:
+        batch's zone map contradicts skips the batch as it would alone; the other queries of its pass run it together."""
+        for g in self.passes:
             if len(g) == 1:
                 self.executors[g[0]].process_batch(batch, stream, time_filters, cutoff)
                 continue

@@ -132,7 +132,9 @@ class AggQuery:
         `measures`: queries sharing this query's dimensions, time filter, joins and reduce mode (shared_scan_key); the
         plan ends with their measure roots, root k (SinkArg k) feeding the k-th state of ExecuteBatchPlanMulti.  The
         filters every one of them carries come first, in this query's order; each query's other filters follow as member
-        filter roots (PLAN_SINK_MEASURE_FILTER, SinkArg k), before the dimensions."""
+        filter roots (PLAN_SINK_MEASURE_FILTER, SinkArg k), before the dimensions.  When their dimensions differ, the plan
+        carries the union of them (member_dimensions) as member dimension roots (PLAN_SINK_MEMBER_DIMENSION, SinkArg = the
+        mask of the queries that group by the dimension)."""
         members = [self] if measures is None else measures
         insts: list[A.PlanInst] = []
         self.foreign_columns = []   # distinct (table, column, timezone) leaves in first-use order = BatchPlan.ForeignColumns
@@ -185,8 +187,12 @@ class AggQuery:
             for f in q.filters:
                 if not any(f == g for g in shared):
                     emit(f, A.PLAN_SINK_MEASURE_FILTER, k, A.Bool)
-        for pos, qi in enumerate(self.dim_order):
-            emit(self.dimensions[qi], A.PLAN_SINK_DIMENSION, pos, self.dim_types[qi])
+        union = member_dimensions(members)
+        if union is None:
+            for pos, qi in enumerate(self.dim_order):
+                emit(self.dimensions[qi], A.PLAN_SINK_DIMENSION, pos, self.dim_types[qi])
+        for e, dt, mask in union or ():
+            emit(e, A.PLAN_SINK_MEMBER_DIMENSION, mask, dt)
         for k, q in enumerate(members):
             emit(q.measure, A.PLAN_SINK_MEASURE, k, q.measure_data_type)
         if len(insts) > A.ARES_MAX_PLAN_INSTS:
@@ -209,6 +215,35 @@ class AggQuery:
             return dims, repr(self.filters[lo:hi]), joins, self.reduce_mode
         prefix = tuple(bytes(pi) for pi in self.plan_instructions(measures=[]))
         return prefix, self.time_filter_range, joins, self.reduce_mode
+
+
+def member_dimensions(queries: list):
+    """The union of the dimensions of `queries` as (expression, output data type, mask of the queries that have it), or
+    None when they all have the same dimensions.  Dimensions compare structurally, with their type; the union is ordered
+    so that every query's dimensions appear in its own layout order (dim_order), each new dimension as early as that
+    allows.  Raises ValueError when no such order exists (two queries order two dimensions of the same width
+    differently)."""
+    seqs = [[repr((q.dimensions[qi], q.dim_types[qi])) for qi in q.dim_order] for q in queries]
+    if all(s == seqs[0] for s in seqs):
+        return None
+    info, order = {}, []
+    for q, s in zip(queries, seqs):
+        for key, qi in zip(s, q.dim_order):
+            if key not in info:
+                info[key] = (q.dimensions[qi], q.dim_types[qi])
+                order.append(key)
+    pos, out = [0] * len(seqs), []
+    while len(out) < len(order):
+        # a dimension comes next when it is the next one of every query that has it
+        nxt = next((key for key in order if key not in out and
+                    all(key not in s or (pos[k] < len(s) and s[pos[k]] == key) for k, s in enumerate(seqs))), None)
+        if nxt is None:
+            raise ValueError("the queries order their dimensions differently")
+        out.append(nxt)
+        for k, s in enumerate(seqs):
+            if pos[k] < len(s) and s[pos[k]] == nxt:
+                pos[k] += 1
+    return [(*info[key], sum(1 << k for k, s in enumerate(seqs) if key in s)) for key in out]
 
 
 class QueryResult:

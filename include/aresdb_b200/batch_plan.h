@@ -59,8 +59,11 @@ enum PlanSink {
   PLAN_SINK_DIMENSION = 2, /* root of dimension #SinkArg (layout order), DimensionOutput         */
   PLAN_SINK_MEASURE = 3,   /* root of the measure, MeasureOutput of SinkDataType / AggSpec.AggFunc; ExecuteBatchPlanMulti:
                             * one root per state, SinkArg = the ordinal of the state it feeds */
-  PLAN_SINK_MEASURE_FILTER = 4 /* ExecuteBatchPlanMulti only: root of a filter that applies to state SinkArg alone (a
-                                * member filter, see ExecuteBatchPlanMulti) */
+  PLAN_SINK_MEASURE_FILTER = 4, /* ExecuteBatchPlanMulti only: root of a filter that applies to state SinkArg alone (a
+                                 * member filter, see ExecuteBatchPlanMulti) */
+  PLAN_SINK_MEMBER_DIMENSION = 5 /* ExecuteBatchPlanMulti only: root of a dimension of the states whose bits are set in
+                                  * SinkArg (bit k = state k); its ordinal in state k's layout is its position among the
+                                  * member dimension roots with bit k (a member dimension, see ExecuteBatchPlanMulti) */
 };
 
 typedef struct {
@@ -68,7 +71,7 @@ typedef struct {
   uint8_t Functor;
   uint8_t Sink;         /* enum PlanSink */
   uint8_t SinkArg;      /* dimension ordinal for PLAN_SINK_DIMENSION; state ordinal for PLAN_SINK_MEASURE and
-                         * PLAN_SINK_MEASURE_FILTER (Multi) */
+                         * PLAN_SINK_MEASURE_FILTER (Multi); mask of states for PLAN_SINK_MEMBER_DIMENSION (Multi) */
   uint8_t SinkDataType; /* enum DataType of the sink element */
   uint8_t Reserved[3];
   PlanOperand A;
@@ -176,7 +179,27 @@ CGoCallResHandle ExecuteBatchPlan(void *state, const BatchPlan *plan, void *cuda
  * filter roots out of that order.  In the one-kernel form a row's dimensions are computed when it is alive for some
  * state, and each state's accumulators see only the rows alive for it; in the per-state form state k runs its
  * single-measure plan, which keeps state k's member filters as ordinary filters and drops the other states' member
- * filters.  numStates == 1 is ExecuteBatchPlan of the plan with its member filters turned into filters. */
+ * filters.  numStates == 1 is ExecuteBatchPlan of the plan with its member filters turned into filters.
+ *
+ * Member dimensions: the states may also differ in their dimensions.  Such a plan has no PLAN_SINK_DIMENSION root;
+ * instead every dimension of the union of the states' dimensions is one PLAN_SINK_MEMBER_DIMENSION root whose SinkArg
+ * is the mask of the states that group by it, so that a dimension several states share is evaluated once.  State k's
+ * dimensions are the roots with bit k, in plan order, and their widths must be the layout its NumDimsPerDimWidth
+ * describes (16, 8, 4, 2, 1 bytes); the states may then differ in NumDimsPerDimWidth.  Member dimension roots follow
+ * the member filter roots and precede the measure roots.  Rejected with an error string: a member dimension in a plan
+ * given to ExecuteBatchPlan, a zero mask, a mask bit >= numStates, a plan with both kinds of dimension roots, roots out
+ * of that order, and widths that differ from a state's layout.  The form is chosen per batch, in this order:
+ *   1. one kernel for all states: every state's own plan takes the CTA's direct-indexed slots, their regions (each
+ *      sized by its own slot count) fit a CTA together, and the states agree in key form (rows of at most 8 bytes, or
+ *      rows of the same length); a row's index in every union dimension is computed once, and each state's slot is
+ *      derived from the indexes of its own dimensions;
+ *   2. otherwise one ExecuteBatchPlanMulti per set of states with identical dimensions (the plan of that set: its
+ *      measure and member filter roots, its dimensions as PLAN_SINK_DIMENSION roots), each deciding its form as above;
+ *   3. when no such set takes a direct-indexed form, that is one kernel per state.
+ * Every state gets exactly the result it gets alone.  A caller builds the union from the states' dimension
+ * expressions, compared structurally together with their output type: each state's dimensions must appear in the
+ * union in its own layout order, which is possible unless two states order two dimensions of the same width
+ * differently (such states belong in separate calls). */
 CGoCallResHandle ExecuteBatchPlanMulti(void *const *states, int numStates, const BatchPlan *plan, void *cudaStream, int device);
 
 /* Folds already-reduced rows (a DimensionVector block + measure vector, e.g. the carried

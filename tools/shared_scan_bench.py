@@ -2,8 +2,11 @@
 """The cfg3 table (8 day-batches x 1.25e8 rows, zone maps) queried by one dashboard request: {sum(fare), count(*)},
 a four-measure request {sum(fare), count(*), avg(fare), max(city_id)}, and a request whose queries differ in their filters
 (common part: the time range and city_id != 0; members: sum(fare) where status = 1 and fare > 5, count(*) where
-status = 1, count(*) where status = 2, count(*)), each run in one pass (FusedRequestExecutor) and as separate queries (one
-FusedBatchExecutor each), alternating in the same process.  Times are CUDA events around the batches of a step plus the finalize of every query; the results of both forms are compared before anything is timed.
+status = 1, count(*) where status = 2, count(*)), and a request whose queries differ in their dimensions (all with the cfg3
+filters: sum(fare) by hour x city, count(*) by hour, count(*) by city, count(*) by status), each run in one pass
+(FusedRequestExecutor) and as separate queries (one FusedBatchExecutor each), alternating in the same process; a request
+of several groups of queries with the same dimensions is also run as it grouped before such groups shared a pass (one
+FusedRequestExecutor per group).  Times are CUDA events around the batches of a step plus the finalize of every query; the results of both forms are compared before anything is timed.
 Usage: python tools/shared_scan_bench.py [--steps N] [--batches B] [--rows R]"""
 import argparse
 import json
@@ -40,7 +43,9 @@ def main():
     requests = {"sum_count": [AggQuery(base.filters, dims, m) for m in ms[:2]],
                 "four_measures": [AggQuery(base.filters, dims, m) for m in ms],
                 "differing_filters": [AggQuery(base.filters, dims, ms[0]), AggQuery([status1] + rest, dims, ms[1]),
-                                      AggQuery([status2] + rest, dims, ms[1]), AggQuery(rest, dims, ms[1])]}
+                                      AggQuery([status2] + rest, dims, ms[1]), AggQuery(rest, dims, ms[1])],
+                "differing_dimensions": [AggQuery(base.filters, d, m) for d, m in
+                                         ((dims, ms[0]), (dims[:1], ms[1]), (dims[1:], ms[1]), ([bench._columns()[2]], ms[1]))]}
     keep, batches = [], []
     for d in range(args.batches):
         bufs, voff = synth.generate_batch_cuda(d, args.rows, dev)
@@ -49,26 +54,35 @@ def main():
         batches.append(Batch(cols, args.rows, ranges=synth.zone_map_of_day(d)))
     torch.cuda.synchronize()
 
-    def results(kind, qs):
+    def executors(kind, qs):
+        """(executors, indexes of the queries each one runs): the whole request, one per group, or one per query."""
         if kind == "shared":
-            ex = FusedRequestExecutor(lib, space, qs)
-            run = [ex]
-        else:
-            run = [FusedBatchExecutor(lib, space, q) for q in qs]
+            return [FusedRequestExecutor(lib, space, qs)], [list(range(len(qs)))]
+        if kind == "per_group":
+            groups = shared_scan_groups(qs, member_filters=True)
+            return [FusedRequestExecutor(lib, space, [qs[i] for i in g]) for g in groups], groups
+        return [FusedBatchExecutor(lib, space, q) for q in qs], [[i] for i in range(len(qs))]
+
+    def collect(run, idx):
+        out = {}
+        for ex, g in zip(run, idx):
+            out.update(zip(g, ex.results() if isinstance(ex, FusedRequestExecutor) else [ex.result()]))
+        return [out[i] for i in range(len(out))]
+
+    def results(kind, qs):
+        run, idx = executors(kind, qs)
         for b in batches:
             for ex in run:
                 ex.process_batch(b)
-        out = ex.results() if kind == "shared" else [ex.result() for ex in run]
+        out = collect(run, idx)
         for ex in run:
             ex.close()
         return out
 
     def timed(kind, qs):
-        ex = FusedRequestExecutor(lib, space, qs) if kind == "shared" else None
-        solos = None if ex else [FusedBatchExecutor(lib, space, q) for q in qs]
+        run, idx = executors(kind, qs)
         times = []
         for step in range(args.steps + 1):   # step 0: warm-up (kernel compile, first launches)
-            run = [ex] if ex else solos
             for e in run:
                 e.reset()
             torch.cuda.synchronize()
@@ -77,12 +91,12 @@ def main():
             for b in batches:
                 for e in run:
                     e.process_batch(b)
-            _ = ex.results() if ex else [x.result() for x in solos]
+            _ = collect(run, idx)
             e_.record()
             torch.cuda.synchronize()
             if step:
                 times.append(s.elapsed_time(e_))
-        for e in ([ex] if ex else solos):
+        for e in run:
             e.close()
         return times
 
@@ -90,25 +104,30 @@ def main():
                          capture_output=True, text=True).stdout.strip()
     report = {"gpu": smi, "rows": args.rows * args.batches, "batches": args.batches, "steps": args.steps, "requests": {}}
     for name, qs in requests.items():
-        shared, separate = results("shared", qs), results("separate", qs)
-        for q, a, b in zip(qs, shared, separate):
-            assert a.rows == b.rows and a.groups == b.groups, f"{name}: groups differ"
-            if q.agg_func == A.AGGR_AVG_FLOAT:
-                assert a.counts.tolist() == b.counts.tolist()
-                np.testing.assert_allclose(a.measures, b.measures, rtol=2e-5, atol=1e-6)
-            else:
-                assert a.measures.tobytes() == b.measures.tobytes(), f"{name}: {q.measure_kind} differs"
-        t = {"shared": [], "separate": []}
-        for _ in range(2):   # alternate the two forms
-            t["shared"] += timed("shared", qs)
-            t["separate"] += timed("separate", qs)
+        kinds = ["shared", "separate"] + (["per_group"] if len(shared_scan_groups(qs, member_filters=True)) > 1 else [])
+        shared = results("shared", qs)
+        for kind in kinds[1:]:
+            for q, a, b in zip(qs, shared, results(kind, qs)):
+                assert a.rows == b.rows and a.groups == b.groups, f"{name} ({kind}): groups differ"
+                if q.agg_func == A.AGGR_AVG_FLOAT:
+                    assert a.counts.tolist() == b.counts.tolist()
+                    np.testing.assert_allclose(a.measures, b.measures, rtol=2e-5, atol=1e-6)
+                else:
+                    assert a.measures.tobytes() == b.measures.tobytes(), f"{name} ({kind}): {q.measure_kind} differs"
+        t = {k: [] for k in kinds}
+        for _ in range(2):   # alternate the forms
+            for k in kinds:
+                t[k] += timed(k, qs)
         med = {k: float(np.median(v)) for k, v in t.items()}
-        report["requests"][name] = {"measures": len(qs), "groups": shared_scan_groups(qs, member_filters=True),
-                                    "shared_ms": med["shared"], "separate_ms": med["separate"],
-                                    "shared_ms_all": t["shared"], "separate_ms_all": t["separate"],
-                                    "speedup": med["separate"] / med["shared"], "results_equal": True}
+        entry = {"measures": len(qs), "groups": shared_scan_groups(qs, member_filters=True), "results_equal": True,
+                 "speedup": med["separate"] / med["shared"]}
+        for k in kinds:
+            entry[f"{k}_ms"], entry[f"{k}_ms_all"] = med[k], t[k]
+            entry[f"{k}_spread_ms"] = float(np.max(t[k]) - np.min(t[k]))
+        report["requests"][name] = entry
+        extra = f", per group {med['per_group']:.2f} ms" if "per_group" in med else ""
         print(f"{name}: one pass {med['shared']:.2f} ms, separate queries {med['separate']:.2f} ms "
-              f"(x{med['separate'] / med['shared']:.2f}), {args.rows * args.batches:.3g} rows, {smi}", flush=True)
+              f"(x{med['separate'] / med['shared']:.2f}){extra}, {args.rows * args.batches:.3g} rows, {smi}", flush=True)
     print(json.dumps(report))
 
 
