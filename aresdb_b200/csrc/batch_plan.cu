@@ -1050,10 +1050,10 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P, Agg
           if (stateFed[pi.SinkArg]) throw EngineError("two measure roots feed state " + std::to_string(pi.SinkArg) + " (duplicate SinkArg)");
           stateFed[pi.SinkArg] = true;
           fed = multi[pi.SinkArg];
-          P.meas[pi.SinkArg].inst = (int8_t)i;
         } else if (measureSeen) {
           throw EngineError("only one measure per plan");
         }
+        P.meas[multi ? pi.SinkArg : 0].inst = (int8_t)i;
         measureSeen = true;
         if (firstDimOrMeasure < 0) firstDimOrMeasure = i;
         if (firstMeasure < 0) firstMeasure = i;
@@ -1163,9 +1163,13 @@ static bool stagesBaseCounts(const DevPlan &P) {
   return !P.skipCount || anyRle;
 }
 
-// Decides the tile size, the stage layout, the TMA ring depth and the shared table size.  The shared table gets what the
-// workload needs first (a table that overflows sends rows to contended L2 atomics, tools/microbench/agg_microbench.cu),
-// the ring takes the rest.  Staged parts must start on a 16-byte boundary (executePlan copies those that do not).
+// What a laid-out single-measure plan decided for its measure (denseFx: it takes the exact-integer form), as the kernel's
+// per-measure code takes it: for the plan itself, or for a state's measure in a shared plan (planShared).
+static void describeMeasure(const DevPlan &Q, DevMeasure &M) {
+  M.aggOp = Q.aggOp; M.measWidth = Q.measWidth; M.skipCount = Q.skipCount; M.neutralSafe = Q.neutralSafe;
+  M.denseFx = Q.denseFx; M.fxShift = Q.fxShift; M.measureIdentity = Q.measureIdentity; M.accNeutral = Q.accNeutral;
+}
+
 // Member dimensions: the slots of each measure's region when `avail` bytes of shared memory hold them, false when they do
 // not.  Each region holds at least the measure's own slots; the rest of `avail` is shared in proportion to them (for
 // lane-private copies of few slots).
@@ -1191,6 +1195,10 @@ static bool memberSlots(DevPlan &P, size_t avail) {
   return true;
 }
 
+// Decides the tile size, the stage layout, the TMA ring depth and the shared table size.  The shared table gets what the
+// workload needs first (a table that overflows sends rows to contended L2 atomics, tools/microbench/agg_microbench.cu),
+// the ring takes the rest.  Staged parts must start on a 16-byte boundary (executePlan copies those that do not).
+// A single-measure plan describes its measure in meas[0].
 static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
   const bool stageBc = stagesBaseCounts(P);
   // The shared table takes 8192 slots (128 KB) whenever a ring of >= 2 stages still fits beside
@@ -1255,7 +1263,7 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
       for (uint32_t tr : {3968u, 1920u, 896u}) {
         const uint32_t n = stagesIn((size_t)kSmemBudget - 128 - 256, tr);
         if (n >= 2) {
-          tileRows = tr; stages = n; slots = 16; P.denseGlobal = 1;
+          tileRows = tr; stages = n; slots = 16; P.denseGlobal = 1; P.denseFx = 0;
           // L2 atomics saturate at >= ~1M distinct addresses and contend below (tools/microbench/agg_microbench.cu):
           // replicate the slot array until it has about that many
           uint32_t reps = 1;
@@ -1267,7 +1275,7 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
     }
     // no layout holds the slots, or a batch without a full tile (all of it is the tail, which one CTA folds): hash table
     if (tileRows && fullTiles(tileRows) == 0) { tileRows = 0; slots = 8192; }
-    if (!tileRows) { P.denseNd = 0; P.denseGlobal = 0; }
+    if (!tileRows) { P.denseNd = 0; P.denseGlobal = 0; P.denseFx = 0; }
   }
   if (!tileRows && P.nmeas > 1) { P.denseNd = 0; return 0; }   // several measures share only the CTA's direct-indexed slots
   if (!tileRows) {
@@ -1315,6 +1323,8 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
     P.tableBytes = 0;
     for (int m = 0; m < P.nmeas; m++)
       P.tableBytes += ((P.memberDims ? P.meas[m].slots : slots) * (P.meas[m].denseFx ? 12 : 9) + 127) / 128 * 128;
+  } else {
+    describeMeasure(P, P.meas[0]);
   }
   return 128 + (size_t)P.tableBytes + stageBytes * P.numStages;
 }
@@ -1554,6 +1564,19 @@ static int launchGrid(const DevPlan &P) {
   return grid;
 }
 
+// Launches the kernel of a laid-out plan whose measures feed sts[0..n).  Direct-indexed kernels are not waited for (see
+// "growth of the group table"): what their flush may insert (the CTA slots; the global slot array's fold) is reserved in
+// every state's table up front, and their out-of-range rows park.  Hash-table kernels are checked by the caller.
+static void launchPlan(DevPlan &P, AggState *const *sts, int n, cudaStream_t s) {
+  for (int k = 0; k < n; k++) {
+    if (P.denseNd != 0) ensureRoom(sts[k], (uint64_t)(P.memberDims ? P.meas[k].total : P.denseTotal), s);
+    P.meas[k].G = sts[k]->table;      // (after a possible growth: the slices live in the table's allocation)
+    P.meas[k].ctaAcc = sts[k]->ctaAcc;
+  }
+  P.ctaAcc = sts[0]->ctaAcc;
+  jitLaunch(P, sts[0]->table, 128 + (size_t)P.tableBytes + (size_t)P.stageBytes * P.numStages, launchGrid(P), s);
+}
+
 static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
   if (bp.NumRows == 0) return;
   if (bp.NumRows > 0x7FFFFFFFu) throw EngineError("a batch holds at most 2^31-1 rows");
@@ -1564,15 +1587,10 @@ static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
   prepareInputs(P, bp, s, &scratch);
   std::unique_ptr<Scratch> joinMem;
   uploadJoin(P, bp, s, joinMem);
-  size_t smemBytes = layoutStages(P, st->spec.ExpectedGroups);
+  layoutStages(P, st->spec.ExpectedGroups);
   rleTileHints(P, bp, s, scratch);
-  // room in the group table (see "growth of the group table"): the direct-indexed kernels are not waited for, so what
-  // they may insert is reserved up front (flush of the CTA slots / fold of the global slot array; out-of-range rows
-  // park); hash-table kernels are checked after the launch and resumed when they stopped.
+  // hash-table kernels are checked after the launch and resumed when they stopped
   const bool resumable = P.denseNd == 0 && !st->hllDense;
-  if (!resumable && !st->hllDense) ensureRoom(st, (uint64_t)P.denseTotal, s);
-  P.ctaAcc = st->ctaAcc;   // (after a possible growth: the slices live in the table's allocation)
-  const int grid = launchGrid(P);
   if (P.denseGlobal) {
     if (!st->denseAcc) {   // first use: 16 MB of accumulators at the neutral element (denseFoldKernel leaves them so)
       st->denseAcc = static_cast<unsigned long long *>(deviceAllocOrThrow((size_t)kGlobalDenseMaxSlots * sizeof(unsigned long long)));
@@ -1582,7 +1600,7 @@ static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
     P.denseAcc = st->denseAcc;
   }
   for (;;) {
-    jitLaunch(P, st->table, smemBytes, grid, s);
+    launchPlan(P, &st, 1, s);
     if (P.denseGlobal) {
       DenseFold F;
       memset(&F, 0, sizeof(F));
@@ -1622,7 +1640,6 @@ static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
     settleTable(st, s);   // grows (a quarter full at most afterwards) and folds the parked groups
     if (!stopped) return;
     P.resume = 1;
-    P.ctaAcc = st->ctaAcc;
   }
 }
 
@@ -1732,9 +1749,7 @@ static bool planShared(AggState *const *sts, int n, const BatchPlan &bp, DevPlan
     prepareInputs(Q, subs[k], nullptr, nullptr);
     layoutStages(Q, sts[k]->spec.ExpectedGroups);
     shared = shared && Q.denseNd != 0 && !Q.denseGlobal;
-    DevMeasure &M = P.meas[k];
-    M.aggOp = Q.aggOp; M.measWidth = Q.measWidth; M.skipCount = Q.skipCount; M.neutralSafe = Q.neutralSafe;
-    M.denseFx = Q.denseFx; M.fxShift = Q.fxShift; M.measureIdentity = Q.measureIdentity; M.accNeutral = Q.accNeutral;
+    describeMeasure(Q, P.meas[k]);
     skipCount = skipCount && Q.skipCount;
     // member dimensions: every state packs its rows with the kernel's one key form (JIT_KW / JIT_ROW_BYTES)
     if (P.memberDims && (sts[k]->keyMode != sts[0]->keyMode ||
@@ -1805,16 +1820,8 @@ static void executePlanMulti(AggState *const *sts, int n, const BatchPlan &bp, c
   P.resume = 0;
   std::unique_ptr<Scratch> joinMem;
   uploadJoin(P, bp, s, joinMem);
-  const size_t smemBytes = 128 + (size_t)P.tableBytes + (size_t)P.stageBytes * P.numStages;
   rleTileHints(P, bp, s, scratch);
-  // direct-indexed kernels are not waited for: every state gets room for what the flush may insert up front
-  for (int k = 0; k < n; k++) {
-    ensureRoom(sts[k], (uint64_t)(P.memberDims ? P.meas[k].total : P.denseTotal), s);
-    P.meas[k].G = sts[k]->table;
-    P.meas[k].ctaAcc = sts[k]->ctaAcc;
-  }
-  P.ctaAcc = sts[0]->ctaAcc;
-  jitLaunch(P, sts[0]->table, smemBytes, launchGrid(P), s);
+  launchPlan(P, sts, n, s);
 }
 
 static void mergeRows(AggState *st, const DimensionVector &in, const uint8_t *values, int length, cudaStream_t s) {

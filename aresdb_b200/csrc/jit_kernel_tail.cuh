@@ -3,9 +3,21 @@
 // CTA-private shared table, and the flush into the global table.  The shape macros
 // (JIT_TILE_ROWS, JIT_STAGE_BYTES, JIT_SMEM_SLOTS, JIT_KW, JIT_AGG_OP, JIT_HASH_BITS,
 // JIT_ROW_BYTES, JIT_THREADS, JIT_NUM_PARTS + kPartSmemOff/kPartBytes/kPartTileStride) and
-// rowEval() precede this text.  JIT_NMEAS > 1: the plan's measure roots feed that many states (direct-indexed form).
+// rowEval() precede this text.  JIT_NMEAS > 1: the plan's measure roots feed that many states (direct-indexed form), and
+// the shape describes each measure's form in kMeas* tables (kMeasOp, kMeasAcc, kMeasFlags, kMeasCheck, kMeasSmemOff).
+// A plan with one measure takes them from its own JIT_AGG_OP / JIT_DENSE_* macros, here; the global slot array
+// (JIT_DENSE 2) has no flags.
 #ifndef JIT_NMEAS
 #define JIT_NMEAS 1
+#define JIT_MEAS_REST(v, w)
+#define JIT_MEAS_REST1(v)
+namespace aresb {
+__device__ constexpr int kMeasOp[1] = {JIT_AGG_OP};
+__device__ constexpr int kMeasAcc[1] = {JIT_DENSE_ACC};
+__device__ constexpr bool kMeasFlags[1] = {JIT_DENSE != 2 && JIT_DENSE_FLAGS};
+__device__ constexpr bool kMeasCheck[1] = {JIT_DENSE_CHECK};
+__device__ constexpr uint32_t kMeasSmemOff[1] = {0};
+}  // namespace aresb
 #endif
 // Plans with member filters (PLAN_SINK_MEASURE_FILTER) define JIT_LIVE_ARG(x) as `, x`: their evaluators then report in
 // live[M] the rows alive for measure M.  Without, every measure takes every alive row (live[M] stays 0xF).
@@ -51,57 +63,23 @@ __device__ __forceinline__ unsigned long long jitKeyOf(const uint64_t (&key)[4][
 
 #if JIT_DENSE
 // ---- direct-indexed aggregation (zone map known for every dimension, see jit.cu) --------------------
-// Quads the fast path could not finish — out of line, rare.  The fast path only says WHICH rows were inside the zone map
-// (inRange) and at which slots; everything else is recomputed here with full generality (rowEvalGeneric: alive mask,
-// packed key, converted measure), so that the fast path keeps no masks, keys or doubles alive:
-//   * alive rows outside the ranges (or a NULL whose stored value is not the canonical zero): the global hash table, keyed
-//     like every other path (new groups park in the spill list while the table is at its growth threshold);
-//   * rows inside whose value would leave a flag-less slot at its neutral element: the hash table as well;
-//   * integer form: rows inside whose value is off the 2^-S grid: added in double on the CTA's L2 slice at `slot`
-//     (-0.0, which would leave that half at its neutral element: the hash table).
-#if JIT_NMEAS == 1
-static __device__ __noinline__ void denseColdRows(const uint8_t *stage, uint32_t q, uint32_t row0, const JitParams &P, uint32_t nvalid,
-                                                  uint32_t inRange, uint32_t s0, uint32_t s1, uint32_t s2, uint32_t s3,
-                                                  unsigned long long *tAcc) {
-  uint64_t key[4][JIT_KW], meas[4];
-  const uint32_t slot[4] = {s0, s1, s2, s3};
-  uint32_t alive = rowEvalGeneric(stage, q, row0, P, key, meas);
-  alive &= (1u << nvalid) - 1u;
-#pragma unroll
-  for (int r = 0; r < 4; r++) {
-    if (!((alive >> r) & 1u)) continue;
-    bool toHash = !((inRange >> r) & 1u);
-    if (!toHash) {
-      if (JIT_DENSE_ACC == 4 && JIT_DENSE != 2) {
-        const float x = (float)__longlong_as_double((long long)meas[r]);   // the measure is a float32 widened exactly
-        const float y = x * P.fxScale;
-        const bool onGrid = x > 0.0f && y < 4294967296.0f && __uint2float_rn(__float2uint_rz(y)) == y;
-        if (onGrid) continue;                                   // the fast path added its pieces
-        if (meas[r] != 0x8000000000000000ull) { aggAtomic((AggOp)JIT_AGG_OP, tAcc + slot[r], meas[r]); continue; }
-        toHash = true;                                          // -0.0
-      } else {
-        if (JIT_DENSE != 2 && JIT_DENSE_FLAGS) continue;        // flagged slots take every value
-        if (!JIT_DENSE_CHECK || meas[r] != P.accNeutral) continue;   // the fast path handled it
-        toHash = true;
-      }
-    }
-    if (toHash) globalUpdate(P.G, (AggOp)JIT_AGG_OP, jitKeyOfRow(key[r]), JIT_KW == 1 ? nullptr : key[r], meas[r], /*spillWhenStopped=*/true);
-  }
-}
-#endif
-
-// Where the accumulators of the direct-indexed slots live (JIT_DENSE_ACC, chosen by the host):
+// A row is evaluated once (filters, dimensions, slot); measure M's value goes to its own accumulators: region
+// kMeasSmemOff[M] of the table area (three 32-bit piece counters per slot, or a flag byte per slot followed by 8-byte
+// accumulators), the CTA's slice of its state's ctaAcc, and — for rows the fast path cannot finish — its state's group
+// table.  Each measure keeps the form its single-measure plan takes (kMeasAcc / kMeasFlags / kMeasCheck, chosen by the
+// host).  Where the accumulators of a measure's slots live (kMeasAcc):
 //   1  shared memory (native ATOMS): 4-byte aggregates other than float min / max;
 //   2  the others: row positions 0-1 of a quad go to shared memory (a CAS loop), 2-3 to the CTA's private slice of
 //      global memory (fire-and-forget RED), so that neither the SM's shared-memory atomic path nor its global-atomic
 //      path carries the whole stream; the flush adds the two halves;
 //   4  exact integer accumulation of a bounded float sum (three 32-bit counters per slot).
+// STEP(M) for every measure M (indexes past JIT_NMEAS fold to 0 in code that never runs)
+#define JIT_EACH_MEASURE(STEP) { STEP(0) if (JIT_NMEAS > 1) { STEP((JIT_NMEAS > 1 ? 1 : 0)) } if (JIT_NMEAS > 2) { STEP((JIT_NMEAS > 2 ? 2 : 0)) } if (JIT_NMEAS > 3) { STEP((JIT_NMEAS > 3 ? 3 : 0)) } }
 constexpr uint32_t kDenseCap = JIT_SMEM_SLOTS;   // a multiple of 16; JIT_TABLE_BYTES >= 9 * kDenseCap
-// layout of the table region (dynamic shared memory + 128) in this mode: touched[kDenseCap] | acc[kDenseCap] (8 bytes each)
-__device__ __forceinline__ unsigned long long *denseSharedAcc() {
-  extern __shared__ __align__(128) uint8_t denseSmem[];
-  return reinterpret_cast<unsigned long long *>(denseSmem + 128 + kDenseCap);
-}
+// Unit of the fast path's slot offsets (dslot, repOff): bytes for the integer form of a one-measure plan, whose strides
+// are pre-multiplied by the 12-byte slot (JitParams::dStrideB: one multiply-add per dimension per row and nothing else);
+// slots otherwise (measures of several forms share the slot index).
+constexpr uint32_t kSlotUnit = JIT_NMEAS == 1 && kMeasAcc[0] == 4 ? 12u : 1u;
 
 // predicated single-instruction updates (no branch, no reconvergence point around them)
 __device__ __forceinline__ void stsFlag(uint32_t addr, bool p) {
@@ -151,7 +129,7 @@ __device__ __forceinline__ uint8_t *denseSmemBase() {
 
 // Dense-register HLL, rows the map could not serve (`unknown`: inside the zone map, slot not resolved yet) or that lie
 // outside the zone map: the group's directory slot is found the general way; resolved slots are entered into the map.
-static __device__ __noinline__ void denseColdRowsHll(const uint8_t *stage, uint32_t q, uint32_t row0, const JitParams &P, uint32_t nvalid,
+static __device__ __noinline__ void denseHllColdRows(const uint8_t *stage, uint32_t q, uint32_t row0, const JitParams &P, uint32_t nvalid,
                                                      uint32_t inRange, uint32_t unknown, uint32_t s0, uint32_t s1, uint32_t s2, uint32_t s3) {
 #if JIT_HLL == 2
   uint64_t key[4][JIT_KW], meas[4];
@@ -172,121 +150,6 @@ static __device__ __noinline__ void denseColdRowsHll(const uint8_t *stage, uint3
 #endif
 }
 
-// `repOff`: this lane's copy of the slots (few slots are replicated per lane), in slots — loop invariant, computed once.
-#if JIT_NMEAS == 1
-__device__ __forceinline__ void jitAggregateDense(uint32_t touchedAddr, unsigned long long *tAcc, const JitParams &P, const uint8_t *stage,
-                                                  uint32_t q, uint32_t row0, uint32_t nvalid, uint32_t repOff, const bool (&fast)[4],
-                                                  bool cold, const uint32_t (&dslot)[4], const uint64_t (&meas)[4],
-                                                  const uint32_t (&mraw)[4]) {
-  // slots: dslot + this lane's copy.  (Integer form: dslot arrives in BYTES — strides pre-multiplied by the 12-byte slot —
-  // and so does repOff; the slot index is only needed by the cold path.)
-  uint32_t s[4];
-#pragma unroll
-  for (int r = 0; r < 4; r++) s[r] = dslot[r] + repOff;
-  if (JIT_HLL == 2) {
-    // Dense-register HLL addressed by the zone map: the table region is a map slot -> directory slot of the group (whose
-    // 16384 registers live at regs + 16384 * that).  A known slot costs one shared-memory load and one fire-and-forget
-    // RED.MAX; an unknown one (first row of the group in this CTA) goes through denseColdRows, which fills the map.
-    // (the four map entries are read back to back — plain loads: a stale "unknown" only sends the row to the cold path,
-    // which resolves the slot again — and only then the four updates are issued)
-    const uint32_t *map = reinterpret_cast<const uint32_t *>(denseSmemBase());
-    asm volatile("" ::: "memory");
-    uint32_t ds[4];
-#pragma unroll
-    for (int r = 0; r < 4; r++) ds[r] = map[fast[r] ? s[r] : 0u];
-    // (register index in 32 bits — the dense directory has at most 2^18 groups —, the update a PREDICATED red: no branch
-    // around it, and the four addresses are ready before the first one is issued)
-    uint32_t *reg[4];
-#pragma unroll
-    for (int r = 0; r < 4; r++) reg[r] = P.G.regs + ((ds[r] << 14) | ((uint32_t)meas[r] & (kHllRegisters - 1)));
-    static_assert(kHllRegisters == 1u << 14, "register index packing");
-#pragma unroll
-    for (int r = 0; r < 4; r++) {
-      const bool known = fast[r] && ds[r] != 0xFFFFFFFFu;
-      cold = cold || (fast[r] && !known);
-      asm volatile("{ .reg .pred p; setp.ne.u32 p, %0, 0; @p red.global.max.u32 [%1], %2; }"
-                   ::"r"((uint32_t)known), "l"(reg[r]), "r"((uint32_t)meas[r] + 1u) : "memory");
-    }
-    if (cold) {
-      const uint32_t unknown = (fast[0] && ds[0] == 0xFFFFFFFFu ? 1u : 0u) | (fast[1] && ds[1] == 0xFFFFFFFFu ? 2u : 0u) |
-                               (fast[2] && ds[2] == 0xFFFFFFFFu ? 4u : 0u) | (fast[3] && ds[3] == 0xFFFFFFFFu ? 8u : 0u);
-      const uint32_t inRange = (fast[0] ? 1u : 0u) | (fast[1] ? 2u : 0u) | (fast[2] ? 4u : 0u) | (fast[3] ? 8u : 0u);
-      // rows already folded through the map must not be folded again: hand over only unknown-slot and out-of-range rows
-      denseColdRowsHll(stage, q, row0, P, nvalid, inRange, unknown, s[0], s[1], s[2], s[3]);
-    }
-    return;
-  }
-  if (JIT_DENSE == 2) {
-    // One accumulator array for the whole grid (more slots than a CTA holds).  No flags: a slot was reached iff it
-    // differs from the aggregate's neutral element, so a row whose value would leave it there (-0.0 for float sums,
-    // the extreme for min / max) goes down the hash path instead; the host only selects this form for aggregates
-    // that cannot return to the neutral element otherwise.
-#pragma unroll
-    for (int r = 0; r < 4; r++) {
-      const bool f = fast[r] && (!JIT_DENSE_CHECK || meas[r] != P.accNeutral);
-      cold = cold || (fast[r] && !f);
-      redGlobalPred<JIT_AGG_OP>(P.gAcc + s[r], meas[r], f);
-    }
-  } else if (JIT_DENSE_ACC == 4) {
-    // Exact integer accumulation of a float sum (jitAnalyzeDense): a slot is three 32-bit counters for the 11 / 11 / 10
-    // bit pieces of x * 2^S, updated with fire-and-forget adds (nothing returns, nothing spins), and carries no flag —
-    // it was reached iff a counter is non-zero or its double half on the L2 slice left the neutral element.  A row is
-    // taken row by row — decide, then add — so that only one row's predicates are alive at a time: x > 0 on the grid
-    // (y = x * 2^S is an integer below 2^32: float -> u32 -> float gives y back) adds its three pieces.  Everything else
-    // in range (zeros, NULL -> +0.0, negative, off the grid, beyond the announced maximum, NaN, -0.0) is rare and is
-    // finished by denseColdRows.
-#pragma unroll
-    for (int r = 0; r < 4; r++) {
-      const float x = __uint_as_float(mraw[r]);
-      const float y = x * P.fxScale;
-      const uint32_t ix = __float2uint_rz(y);
-      const bool onGrid = fast[r] && x > 0.0f && y < 4294967296.0f && __uint2float_rn(ix) == y;
-      cold = cold || (fast[r] && !onGrid);
-      if (onGrid) {   // one branch around the three adds
-        const uint32_t a = touchedAddr + s[r];
-        asm volatile("red.shared.add.u32 [%0], %1;\n\tred.shared.add.u32 [%0+4], %2;\n\tred.shared.add.u32 [%0+8], %3;"
-                     ::"r"(a), "r"(ix & 0x7FFu), "r"((ix >> 11) & 0x7FFu), "r"(ix >> 22) : "memory");
-      }
-    }
-  } else {
-    bool go[4];
-#pragma unroll
-    for (int r = 0; r < 4; r++) {
-      // no flags: a row that would leave its slot at the neutral element goes down the hash path instead
-      go[r] = fast[r] && (JIT_DENSE_FLAGS || !JIT_DENSE_CHECK || meas[r] != P.accNeutral);
-      cold = cold || (fast[r] && !go[r]);
-    }
-    if (JIT_DENSE_FLAGS) {
-#pragma unroll
-      for (int r = 0; r < 4; r++) stsFlag(touchedAddr + s[r], go[r]);
-    }
-    const uint32_t sAccAddr = touchedAddr + kDenseCap;
-    // (issuing the compare-and-swap loops of the shared-memory rows interleaved instead of one after the other was
-    // measured and changed nothing: 0.376 vs 0.372 ms on cfg3)
-    constexpr int kToShared = JIT_DENSE_ACC == 1 ? 4 : 2;   // row positions 0 .. kToShared-1
-#pragma unroll
-    for (int r = 0; r < 4; r++) {
-      if (r < kToShared) redSharedPred<JIT_AGG_OP>(sAccAddr + 8u * s[r], denseSharedAcc() + s[r], meas[r], go[r]);
-      else redGlobalPred<JIT_AGG_OP>(tAcc + s[r], meas[r], go[r]);
-    }
-  }
-  if (cold) {
-    const uint32_t inRange = (fast[0] ? 1u : 0u) | (fast[1] ? 2u : 0u) | (fast[2] ? 4u : 0u) | (fast[3] ? 8u : 0u);
-    constexpr uint32_t kUnit = JIT_DENSE_ACC == 4 && JIT_DENSE != 2 ? 12u : 1u;   // bytes -> slots
-    denseColdRows(stage, q, row0, P, nvalid, inRange, s[0] / kUnit, s[1] / kUnit, s[2] / kUnit, s[3] / kUnit, tAcc);
-  }
-}
-#endif
-
-#if JIT_NMEAS > 1
-// ---- several measures, one pass (ExecuteBatchPlanMulti) ---------------------------------------------------------------
-// A row is evaluated once (filters, dimensions, slot); measure M's value goes to its own accumulators: region
-// kMeasSmemOff[M] of the table area (three 12-byte piece counters per slot, or a flag byte per slot followed by 8-byte
-// accumulators), the CTA's slice of its state's ctaAcc, and — for rows the fast path cannot finish — its state's group
-// table.  Each measure keeps the form its single-measure plan takes (kMeasAcc / kMeasFlags / kMeasCheck are JIT_DENSE_ACC
-// / JIT_DENSE_FLAGS / JIT_DENSE_CHECK of that plan), with the same rules as jitAggregateDense / denseColdRows.
-// STEP(M) for every measure M (indexes past JIT_NMEAS fold to 0 in code that never runs)
-#define JIT_EACH_MEASURE(STEP) { STEP(0) STEP(1) if (JIT_NMEAS > 2) { STEP((JIT_NMEAS > 2 ? 2 : 0)) } if (JIT_NMEAS > 3) { STEP((JIT_NMEAS > 3 ? 3 : 0)) } }
 template <int M>
 __device__ __forceinline__ unsigned long long *measSlice(const JitParams &P) { return P.ms[M].ctaAcc + (size_t)blockIdx.x * JIT_SMEM_SLOTS; }
 // slots of measure M's region, its dimensions, and the slots its CTA-private copies span
@@ -313,9 +176,17 @@ __device__ __forceinline__ uint32_t measSlots(const JitParams &P, uint32_t dense
 // a quad's slots: one set (shared dimensions) or one per measure (JIT_MDIMS)
 struct JitSlots { uint32_t v[JIT_NSLOT][4]; };
 
+// Quads the fast path could not finish — out of line, rare.  The fast path only says WHICH rows were inside the zone map
+// (inRange) and at which slots; everything else is recomputed here with full generality (rowEvalGeneric: alive mask,
+// packed key, converted measure), so that the fast path keeps no masks, keys or doubles alive:
+//   * alive rows outside the ranges (or a NULL whose stored value is not the canonical zero): the global hash table, keyed
+//     like every other path (new groups park in the spill list while the table is at its growth threshold);
+//   * rows inside whose value would leave a flag-less slot at its neutral element: the hash table as well;
+//   * integer form: rows inside whose value is off the 2^-S grid: added in double on the CTA's L2 slice at `slot`
+//     (-0.0, which would leave that half at its neutral element: the hash table).
 template <int M>
-__device__ __forceinline__ void multiColdMeasure(const JitParams &P, uint32_t alive, uint32_t inRange, const uint64_t (&key)[4][JIT_KW],
-                                                 const uint64_t (&meas)[4], const uint32_t (&slot)[4]) {
+__device__ __forceinline__ void coldMeasure(const JitParams &P, uint32_t alive, uint32_t inRange, const uint64_t (&key)[4][JIT_KW],
+                                            const uint64_t (&meas)[4], const uint32_t (&slot)[4]) {
   constexpr int OP = kMeasOp[M];
   unsigned long long *tAcc = measSlice<M>(P);
 #pragma unroll
@@ -323,12 +194,13 @@ __device__ __forceinline__ void multiColdMeasure(const JitParams &P, uint32_t al
     if (!((alive >> r) & 1u)) continue;
     if ((inRange >> r) & 1u) {
       if (kMeasAcc[M] == 4) {
-        const float x = (float)__longlong_as_double((long long)meas[r]);
+        const float x = (float)__longlong_as_double((long long)meas[r]);   // the measure is a float32 widened exactly
         const float y = x * P.ms[M].fxScale;
         const bool onGrid = x > 0.0f && y < 4294967296.0f && __uint2float_rn(__float2uint_rz(y)) == y;
-        if (onGrid) continue;
+        if (onGrid) continue;                                   // the fast path added its pieces
         if (meas[r] != 0x8000000000000000ull) { aggAtomic((AggOp)OP, tAcc + slot[r], meas[r]); continue; }
       } else {
+        // flagged slots take every value; otherwise the fast path handled every value but the neutral element
         if (kMeasFlags[M] || !kMeasCheck[M] || meas[r] != P.ms[M].accNeutral) continue;
       }
     }
@@ -336,8 +208,8 @@ __device__ __forceinline__ void multiColdMeasure(const JitParams &P, uint32_t al
   }
 }
 
-// the rows some measure's fast path could not finish, evaluated again with full generality (out of line, rare)
-static __device__ __noinline__ void multiColdRows(const uint8_t *stage, uint32_t q, uint32_t row0, const JitParams &P, uint32_t nvalid,
+// the rows some measure's fast path could not finish, evaluated again with full generality; `s`: the quad's slots, in slots
+static __device__ __noinline__ void denseColdQuad(const uint8_t *stage, uint32_t q, uint32_t row0, const JitParams &P, uint32_t nvalid,
                                                   uint32_t inRange, const JitSlots s) {
   uint64_t key[4][JIT_KW], mv[JIT_NMEAS][4];
   uint32_t live[JIT_NMEAS];
@@ -353,18 +225,19 @@ static __device__ __noinline__ void multiColdRows(const uint8_t *stage, uint32_t
 #define JIT_STEP(M) {                                                  \
     uint64_t mkey[4][JIT_KW];                                          \
     _Pragma("unroll") for (int r = 0; r < 4; r++) memberPack<M>(dv[r], dvb[r], mkey[r]); \
-    multiColdMeasure<M>(P, alive & live[M], inRange, mkey, mv[M], s.v[JIT_MDIMS ? M : 0]); }
+    coldMeasure<M>(P, alive & live[M], inRange, mkey, mv[M], s.v[JIT_MDIMS ? M : 0]); }
 #else
-#define JIT_STEP(M) multiColdMeasure<M>(P, alive & live[M], inRange, key, mv[M], s.v[0]);
+#define JIT_STEP(M) coldMeasure<M>(P, alive & live[M], inRange, key, mv[M], s.v[0]);
 #endif
   JIT_EACH_MEASURE(JIT_STEP)
 #undef JIT_STEP
 }
 
-// `live`: the rows of the quad alive for measure M (bit r); `fast` holds the rows alive for some measure inside the zone map
+// `live`: the rows of the quad alive for measure M (bit r); `fastAny` holds the rows alive for some measure inside the
+// zone map; `s`: the slots, in kSlotUnit.  true: some row needs the cold path.
 template <int M>
-__device__ __forceinline__ bool multiDenseMeasure(uint32_t tableAddr, const JitParams &P, const bool (&fastAny)[4], uint32_t live,
-                                                  const uint32_t (&s)[4], const uint64_t (&meas)[4], const uint32_t (&mraw)[4]) {
+__device__ __forceinline__ bool denseMeasure(uint32_t tableAddr, const JitParams &P, const bool (&fastAny)[4], uint32_t live,
+                                             const uint32_t (&s)[4], const uint64_t (&meas)[4], const uint32_t (&mraw)[4]) {
   constexpr int OP = kMeasOp[M];
   const uint32_t base = tableAddr + kMeasSmemOff[M];
   bool cold = false;
@@ -372,6 +245,13 @@ __device__ __forceinline__ bool multiDenseMeasure(uint32_t tableAddr, const JitP
 #pragma unroll
   for (int r = 0; r < 4; r++) fast[r] = fastAny[r] && ((live >> r) & 1u) != 0;
   if (kMeasAcc[M] == 4) {
+    // Exact integer accumulation of a float sum (jitAnalyzeDense): a slot is three 32-bit counters for the 11 / 11 / 10
+    // bit pieces of x * 2^S, updated with fire-and-forget adds (nothing returns, nothing spins), and carries no flag —
+    // it was reached iff a counter is non-zero or its double half on the L2 slice left the neutral element.  A row is
+    // taken row by row — decide, then add — so that only one row's predicates are alive at a time: x > 0 on the grid
+    // (y = x * 2^S is an integer below 2^32: float -> u32 -> float gives y back) adds its three pieces.  Everything else
+    // in range (zeros, NULL -> +0.0, negative, off the grid, beyond the announced maximum, NaN, -0.0) is rare and is
+    // finished by the cold path.
 #pragma unroll
     for (int r = 0; r < 4; r++) {
       const float x = __uint_as_float(mraw[r]);
@@ -379,8 +259,8 @@ __device__ __forceinline__ bool multiDenseMeasure(uint32_t tableAddr, const JitP
       const uint32_t ix = __float2uint_rz(y);
       const bool onGrid = fast[r] && x > 0.0f && y < 4294967296.0f && __uint2float_rn(ix) == y;
       cold = cold || (fast[r] && !onGrid);
-      if (onGrid) {
-        const uint32_t a = base + 12u * s[r];
+      if (onGrid) {   // one branch around the three adds
+        const uint32_t a = base + 12u / kSlotUnit * s[r];
         asm volatile("red.shared.add.u32 [%0], %1;\n\tred.shared.add.u32 [%0+4], %2;\n\tred.shared.add.u32 [%0+8], %3;"
                      ::"r"(a), "r"(ix & 0x7FFu), "r"((ix >> 11) & 0x7FFu), "r"(ix >> 22) : "memory");
       }
@@ -389,6 +269,7 @@ __device__ __forceinline__ bool multiDenseMeasure(uint32_t tableAddr, const JitP
     bool go[4];
 #pragma unroll
     for (int r = 0; r < 4; r++) {
+      // no flags: a row that would leave its slot at the neutral element goes down the hash path instead
       go[r] = fast[r] && (kMeasFlags[M] || !kMeasCheck[M] || meas[r] != P.ms[M].accNeutral);
       cold = cold || (fast[r] && !go[r]);
     }
@@ -398,7 +279,9 @@ __device__ __forceinline__ bool multiDenseMeasure(uint32_t tableAddr, const JitP
     }
     unsigned long long *tAcc = measSlice<M>(P);
     unsigned long long *generic = reinterpret_cast<unsigned long long *>(denseSmemBase() + kMeasSmemOff[M] + measCap<M>());
-    constexpr int kToShared = kMeasAcc[M] == 1 ? 4 : 2;
+    // (issuing the compare-and-swap loops of the shared-memory rows interleaved instead of one after the other was
+    // measured and changed nothing: 0.376 vs 0.372 ms on cfg3)
+    constexpr int kToShared = kMeasAcc[M] == 1 ? 4 : 2;   // row positions 0 .. kToShared-1
 #pragma unroll
     for (int r = 0; r < 4; r++) {
       if (r < kToShared) redSharedPred<OP>(base + measCap<M>() + 8u * s[r], generic + s[r], meas[r], go[r]);
@@ -408,11 +291,12 @@ __device__ __forceinline__ bool multiDenseMeasure(uint32_t tableAddr, const JitP
   return cold;
 }
 
-__device__ __forceinline__ void multiAggregateDense(uint32_t tableAddr, const JitParams &P, const uint8_t *stage, uint32_t q, uint32_t row0,
-                                                    uint32_t nvalid, uint32_t repOff, const bool (&fast)[4], bool cold,
-                                                    const uint32_t (&dslot)[JIT_NSLOT][4], const uint64_t (&mv)[JIT_NMEAS][4],
-                                                    const uint32_t (&mr)[JIT_NMEAS][4], const uint32_t (&live)[JIT_NMEAS]) {
-  // (JIT_MDIMS: each measure's lane-private copy follows its own slot count)
+// `repOff`: this lane's copy of the slots (few slots are replicated per lane), in kSlotUnit — loop invariant, computed once.
+__device__ __forceinline__ void jitAggregateDense(uint32_t tableAddr, const JitParams &P, const uint8_t *stage, uint32_t q, uint32_t row0,
+                                                  uint32_t nvalid, uint32_t repOff, const bool (&fast)[4], bool cold,
+                                                  const uint32_t (&dslot)[JIT_NSLOT][4], const uint64_t (&mv)[JIT_NMEAS][4],
+                                                  const uint32_t (&mr)[JIT_NMEAS][4], const uint32_t (&live)[JIT_NMEAS]) {
+  // slots: dslot + this lane's copy (JIT_MDIMS: each measure's copy follows its own slot count)
   JitSlots s;
 #pragma unroll
   for (int m = 0; m < JIT_NSLOT; m++) {
@@ -420,90 +304,140 @@ __device__ __forceinline__ void multiAggregateDense(uint32_t tableAddr, const Ji
 #pragma unroll
     for (int r = 0; r < 4; r++) s.v[m][r] = dslot[m][r] + off;
   }
-#define JIT_STEP(M) cold = multiDenseMeasure<M>(tableAddr, P, fast, live[M], s.v[JIT_MDIMS ? M : 0], mv[M], mr[M]) || cold;
-  JIT_EACH_MEASURE(JIT_STEP)
+  if (JIT_HLL == 2) {
+    // Dense-register HLL addressed by the zone map: the table region is a map slot -> directory slot of the group (whose
+    // 16384 registers live at regs + 16384 * that).  A known slot costs one shared-memory load and one fire-and-forget
+    // RED.MAX; an unknown one (first row of the group in this CTA) goes through denseHllColdRows, which fills the map.
+    // (the four map entries are read back to back — plain loads: a stale "unknown" only sends the row to the cold path,
+    // which resolves the slot again — and only then the four updates are issued)
+    const uint32_t *map = reinterpret_cast<const uint32_t *>(denseSmemBase());
+    asm volatile("" ::: "memory");
+    uint32_t ds[4];
+#pragma unroll
+    for (int r = 0; r < 4; r++) ds[r] = map[fast[r] ? s.v[0][r] : 0u];
+    // (register index in 32 bits — the dense directory has at most 2^18 groups —, the update a PREDICATED red: no branch
+    // around it, and the four addresses are ready before the first one is issued)
+    uint32_t *reg[4];
+#pragma unroll
+    for (int r = 0; r < 4; r++) reg[r] = P.G.regs + ((ds[r] << 14) | ((uint32_t)mv[0][r] & (kHllRegisters - 1)));
+    static_assert(kHllRegisters == 1u << 14, "register index packing");
+#pragma unroll
+    for (int r = 0; r < 4; r++) {
+      const bool known = fast[r] && ds[r] != 0xFFFFFFFFu;
+      cold = cold || (fast[r] && !known);
+      asm volatile("{ .reg .pred p; setp.ne.u32 p, %0, 0; @p red.global.max.u32 [%1], %2; }"
+                   ::"r"((uint32_t)known), "l"(reg[r]), "r"((uint32_t)mv[0][r] + 1u) : "memory");
+    }
+    if (cold) {
+      const uint32_t unknown = (fast[0] && ds[0] == 0xFFFFFFFFu ? 1u : 0u) | (fast[1] && ds[1] == 0xFFFFFFFFu ? 2u : 0u) |
+                               (fast[2] && ds[2] == 0xFFFFFFFFu ? 4u : 0u) | (fast[3] && ds[3] == 0xFFFFFFFFu ? 8u : 0u);
+      const uint32_t inRange = (fast[0] ? 1u : 0u) | (fast[1] ? 2u : 0u) | (fast[2] ? 4u : 0u) | (fast[3] ? 8u : 0u);
+      // rows already folded through the map must not be folded again: hand over only unknown-slot and out-of-range rows
+      denseHllColdRows(stage, q, row0, P, nvalid, inRange, unknown, s.v[0][0], s.v[0][1], s.v[0][2], s.v[0][3]);
+    }
+    return;
+  }
+  if (JIT_DENSE == 2) {
+    // One accumulator array for the whole grid (more slots than a CTA holds).  No flags: a slot was reached iff it
+    // differs from the aggregate's neutral element, so a row whose value would leave it there (-0.0 for float sums,
+    // the extreme for min / max) goes down the hash path instead; the host only selects this form for aggregates
+    // that cannot return to the neutral element otherwise.
+#pragma unroll
+    for (int r = 0; r < 4; r++) {
+      const bool f = fast[r] && (!JIT_DENSE_CHECK || mv[0][r] != P.accNeutral);
+      cold = cold || (fast[r] && !f);
+      redGlobalPred<JIT_AGG_OP>(P.gAcc + s.v[0][r], mv[0][r], f);
+    }
+  } else {
+#define JIT_STEP(M) cold = denseMeasure<M>(tableAddr, P, fast, live[M], s.v[JIT_MDIMS ? M : 0], mv[M], mr[M]) || cold;
+    JIT_EACH_MEASURE(JIT_STEP)
 #undef JIT_STEP
+  }
   if (cold) {
     const uint32_t inRange = (fast[0] ? 1u : 0u) | (fast[1] ? 2u : 0u) | (fast[2] ? 4u : 0u) | (fast[3] ? 8u : 0u);
-    multiColdRows(stage, q, row0, P, nvalid, inRange, s);
-  }
-}
-
-template <int M>
-__device__ __forceinline__ void multiInitMeasure(const JitParams &P, uint32_t denseSlots) {
-  {
-    uint8_t *base = denseSmemBase() + kMeasSmemOff[M];
-    unsigned long long *tAcc = measSlice<M>(P);
-    const uint32_t n = measSlots<M>(P, denseSlots);
-    for (uint32_t i = threadIdx.x; i < n; i += JIT_THREADS) {
-      if (kMeasAcc[M] != 1) tAcc[i] = P.ms[M].accNeutral;
-      if (kMeasAcc[M] == 4) {
-        uint32_t *c = reinterpret_cast<uint32_t *>(base) + 3u * i;
-        c[0] = 0; c[1] = 0; c[2] = 0;
-      } else {
-        if (kMeasFlags[M]) base[i] = 0;
-        reinterpret_cast<unsigned long long *>(base + measCap<M>())[i] = P.ms[M].accNeutral;
-      }
-    }
-  }
-}
-__device__ __forceinline__ void multiInit(const JitParams &P, uint32_t denseSlots) {
-#define JIT_STEP(M) multiInitMeasure<M>(P, denseSlots);
-  JIT_EACH_MEASURE(JIT_STEP)
-#undef JIT_STEP
-}
-
-// the CTA's slots of every measure into its state's group table (as the single-measure flush)
-template <int M>
-__device__ __forceinline__ void multiFlushMeasure(const JitParams &P, uint32_t denseSlots) {
-  {
-    constexpr int OP = kMeasOp[M];
-    const uint8_t *base = denseSmemBase() + kMeasSmemOff[M];
-    unsigned long long *tAcc = measSlice<M>(P);
-    const unsigned long long neutral = P.ms[M].accNeutral;
-    const uint32_t n = measSlots<M>(P, denseSlots);
-    for (uint32_t i = threadIdx.x; i < n; i += JIT_THREADS) {
-      unsigned long long accS = neutral;
-      if (kMeasAcc[M] == 4) {
-        const uint32_t *c = reinterpret_cast<const uint32_t *>(base) + 3u * i;
-        const unsigned long long v = (unsigned long long)c[0] + ((unsigned long long)c[1] << 11) + ((unsigned long long)c[2] << 22);
-        if (v != 0) accS = (unsigned long long)__double_as_longlong(__ull2double_rn(v) * P.ms[M].fxInv);
-      } else {
-        accS = reinterpret_cast<const unsigned long long *>(base + measCap<M>())[i];
-      }
-      const unsigned long long accG = kMeasAcc[M] != 1 ? __ldcg(&tAcc[i]) : neutral;
-      if (kMeasFlags[M] ? !base[i] : (accS == neutral && accG == neutral)) continue;
-      // (JIT_MDIMS: measure M's slot decodes over its own dimensions and strides)
-      uint32_t rem = i % (JIT_MDIMS ? P.mRepStride[M] : P.dRepStride), dvr[JIT_ND], vb = 0;
 #pragma unroll
-      for (int k = JIT_ND - 1; k >= 0; k--) {
-        dvr[k] = 0u;
-        if (!((measDims<M>() >> k) & 1u)) continue;
-        const uint32_t stride = JIT_MDIMS ? P.mStride[M][k] : P.dStride[k];
-        const uint32_t ix = rem / stride;
-        rem -= ix * stride;
-        const bool valid = ix != P.dCnt[k];
-        dvr[k] = valid ? (P.dLo[k] + ix) * P.dStep[k] : 0u;
-        vb |= (valid ? 1u : 0u) << k;
-      }
-      uint64_t key[JIT_KW];
-#if JIT_MDIMS
-      memberPack<M>(dvr, vb, key);
-#else
-      densePack(dvr, vb, key);
-#endif
-      const unsigned long long k = jitKeyOfRow(key);
-      if (kMeasAcc[M] != 1) globalUpdate<M>(P.ms[M].G, (AggOp)OP, k, JIT_KW == 1 ? nullptr : key, accG, true);
-      globalUpdate<M>(P.ms[M].G, (AggOp)OP, k, JIT_KW == 1 ? nullptr : key, accS, true);
+    for (int m = 0; m < JIT_NSLOT; m++) {
+#pragma unroll
+      for (int r = 0; r < 4; r++) s.v[m][r] /= kSlotUnit;
+    }
+    denseColdQuad(stage, q, row0, P, nvalid, inRange, s);
+  }
+}
+
+template <int M>
+__device__ __forceinline__ void denseInitMeasure(const JitParams &P, uint32_t denseSlots) {
+  uint8_t *base = denseSmemBase() + kMeasSmemOff[M];
+  unsigned long long *tAcc = measSlice<M>(P);
+  const uint32_t n = measSlots<M>(P, denseSlots);
+  for (uint32_t i = threadIdx.x; i < n; i += JIT_THREADS) {
+    if (kMeasFlags[M]) base[i] = 0;   // (flags only in the 9-byte form)
+    if (kMeasAcc[M] != 1) tAcc[i] = P.ms[M].accNeutral;
+    if (kMeasAcc[M] == 4) {
+      uint32_t *c = reinterpret_cast<uint32_t *>(base) + 3u * i;
+      c[0] = 0; c[1] = 0; c[2] = 0;
+    } else {
+      reinterpret_cast<unsigned long long *>(base + measCap<M>())[i] = P.ms[M].accNeutral;
     }
   }
 }
-__device__ __forceinline__ void multiFlush(const JitParams &P, uint32_t denseSlots) {
-#define JIT_STEP(M) multiFlushMeasure<M>(P, denseSlots);
+__device__ __forceinline__ void denseInit(const JitParams &P, uint32_t denseSlots) {
+#define JIT_STEP(M) denseInitMeasure<M>(P, denseSlots);
   JIT_EACH_MEASURE(JIT_STEP)
 #undef JIT_STEP
 }
+
+// the CTA's slots of measure M into its state's group table: the slot index decodes to the dimension values
+template <int M>
+__device__ __forceinline__ void denseFlushMeasure(const JitParams &P, uint32_t denseSlots) {
+  constexpr int OP = kMeasOp[M];
+  const uint8_t *base = denseSmemBase() + kMeasSmemOff[M];
+  unsigned long long *tAcc = measSlice<M>(P);
+  const unsigned long long neutral = P.ms[M].accNeutral;
+  const uint32_t n = measSlots<M>(P, denseSlots);
+  for (uint32_t i = threadIdx.x; i < n; i += JIT_THREADS) {
+    unsigned long long accS = neutral;
+    if (kMeasAcc[M] == 4) {
+      // pieces -> integer -> double: only positive values were added, so 0 = no such row (adding the neutral element
+      // below is then a no-op); 2^-S is a power of two and the integer is exact below 2^53
+      const uint32_t *c = reinterpret_cast<const uint32_t *>(base) + 3u * i;
+      const unsigned long long v = (unsigned long long)c[0] + ((unsigned long long)c[1] << 11) + ((unsigned long long)c[2] << 22);
+      if (v != 0) accS = (unsigned long long)__double_as_longlong(__ull2double_rn(v) * P.ms[M].fxInv);
+    } else {
+      accS = reinterpret_cast<const unsigned long long *>(base + measCap<M>())[i];
+    }
+    const unsigned long long accG = kMeasAcc[M] != 1 ? __ldcg(&tAcc[i]) : neutral;
+    if (kMeasFlags[M] ? !base[i] : (accS == neutral && accG == neutral)) continue;
+    // (JIT_MDIMS: measure M's slot decodes over its own dimensions and strides; padding slots between copies are never
+    // reached)
+    uint32_t rem = i % (JIT_MDIMS ? P.mRepStride[M] : P.dRepStride), dvr[JIT_ND], vb = 0;
+#pragma unroll
+    for (int k = JIT_ND - 1; k >= 0; k--) {
+      dvr[k] = 0u;
+      if (!((measDims<M>() >> k) & 1u)) continue;
+      const uint32_t stride = JIT_MDIMS ? P.mStride[M][k] : P.dStride[k];
+      const uint32_t ix = rem / stride;
+      rem -= ix * stride;
+      const bool valid = ix != P.dCnt[k];
+      dvr[k] = valid ? (P.dLo[k] + ix) * P.dStep[k] : 0u;
+      vb |= (valid ? 1u : 0u) << k;
+    }
+    uint64_t key[JIT_KW];
+#if JIT_MDIMS
+    memberPack<M>(dvr, vb, key);
+#else
+    densePack(dvr, vb, key);
 #endif
+    const unsigned long long k = jitKeyOfRow(key);
+    // (the host does not wait for these kernels: when the table is at its growth threshold new groups are parked)
+    if (kMeasAcc[M] != 1) globalUpdate<M>(P.ms[M].G, (AggOp)OP, k, JIT_KW == 1 ? nullptr : key, accG, true);
+    globalUpdate<M>(P.ms[M].G, (AggOp)OP, k, JIT_KW == 1 ? nullptr : key, accS, true);
+  }
+}
+__device__ __forceinline__ void denseFlush(const JitParams &P, uint32_t denseSlots) {
+#define JIT_STEP(M) denseFlushMeasure<M>(P, denseSlots);
+  JIT_EACH_MEASURE(JIT_STEP)
+#undef JIT_STEP
+}
 #endif
 
 // Folds the surviving rows of one quad.  Normal mode: the CTA's shared table first, the global table
@@ -579,28 +513,14 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
   SmemTable T;
   T.keys = tKeys; T.acc = tAcc; T.claims = claims; T.mask = JIT_SMEM_SLOTS - 1;
 #if JIT_DENSE
-  // no keys: the slot index IS the group; one byte per slot records that a row reached it
-  uint8_t *touched = reinterpret_cast<uint8_t *>(tKeys);
-  uint32_t touchedAddr = smemAddr(touched);
-  asm volatile("" : "+r"(touchedAddr));   // keep it in a register: the compiler otherwise rebuilds the window address per store
+  // no keys: the slot index IS the group; the table area holds each measure's accumulators (and "reached" flags)
+  uint32_t tableAddr = smemAddr(tKeys);
+  asm volatile("" : "+r"(tableAddr));   // keep it in a register: the compiler otherwise rebuilds the window address per store
   const uint32_t denseSlots = JIT_DENSE == 2 ? 0u : P.dRepStride * P.dReps;   // <= kDenseCap (host); 2: nothing CTA-private
-  const uint32_t repOff = JIT_DENSE == 2 ? (blockIdx.x & (P.dReps - 1u)) * P.dRepStride : (threadIdx.x & (P.dReps - 1u)) * P.dRepStride *
-                                                (JIT_DENSE_ACC == 4 && JIT_NMEAS == 1 ? 12u : 1u);   // this lane's copy of the slots (integer form: in bytes)
+  const uint32_t repOff = JIT_DENSE == 2 ? (blockIdx.x & (P.dReps - 1u)) * P.dRepStride
+                                         : (threadIdx.x & (P.dReps - 1u)) * P.dRepStride * kSlotUnit;   // this lane's copy of the slots
   for (uint32_t i = threadIdx.x; JIT_HLL == 2 && i < denseSlots; i += JIT_THREADS) reinterpret_cast<uint32_t *>(tKeys)[i] = 0xFFFFFFFFu;
-#if JIT_NMEAS > 1
-  multiInit(P, denseSlots);
-#else
-  for (uint32_t i = threadIdx.x; JIT_HLL != 2 && i < denseSlots; i += JIT_THREADS) {
-    if (JIT_DENSE_FLAGS) touched[i] = 0;
-    if (JIT_DENSE_ACC != 1) tAcc[i] = P.accNeutral;
-    if (JIT_DENSE_ACC == 4) {
-      uint32_t *c = reinterpret_cast<uint32_t *>(tKeys) + 3u * i;
-      c[0] = 0; c[1] = 0; c[2] = 0;
-    } else {
-      denseSharedAcc()[i] = P.accNeutral;
-    }
-  }
-#endif
+  if (JIT_HLL != 2) denseInit(P, denseSlots);
 #else
   for (uint32_t i = threadIdx.x; i < JIT_SMEM_SLOTS; i += JIT_THREADS) {
     tKeys[i] = kEmptyKey;
@@ -669,8 +589,7 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
       const bool bypass = JIT_BYPASS && !allowClaim && *reinterpret_cast<volatile uint32_t *>(misses) > 4u * JIT_SMEM_SLOTS;
       {
         const uint32_t q = threadIdx.x;
-        uint64_t meas[4];
-#if JIT_DENSE && JIT_NMEAS > 1
+#if JIT_DENSE
         uint32_t dslot[JIT_NSLOT][4];
         bool fast[4], anySlow;
         uint64_t mv[JIT_NMEAS][4];
@@ -678,17 +597,10 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
 #pragma unroll
         for (int m = 0; m < JIT_NMEAS; m++) live[m] = 0xFu;
         if (rowEval(stage, q, t * JIT_TILE_ROWS + q * 4, P, 4u, fast, anySlow, JIT_DSLOT(dslot), mv[0], mr[0] JIT_MEAS_REST(mv, mr) JIT_LIVE_ARG(live)))
-          multiAggregateDense(touchedAddr, P, stage, q, t * JIT_TILE_ROWS + q * 4, 4u, repOff, fast, anySlow, dslot, mv, mr, live);
-        (void)meas; (void)allowClaim; (void)bypass;
-#elif JIT_DENSE
-        uint32_t dslot[4];
-        bool fast[4], anySlow;
-        uint32_t mraw[4];
-        if (rowEval(stage, q, t * JIT_TILE_ROWS + q * 4, P, 4u, fast, anySlow, dslot, meas, mraw))
-          jitAggregateDense(touchedAddr, tAcc, P, stage, q, t * JIT_TILE_ROWS + q * 4, 4u, repOff, fast, anySlow, dslot, meas, mraw);
+          jitAggregateDense(tableAddr, P, stage, q, t * JIT_TILE_ROWS + q * 4, 4u, repOff, fast, anySlow, dslot, mv, mr, live);
         (void)allowClaim; (void)bypass;
 #else
-        uint64_t key[4][JIT_KW];
+        uint64_t meas[4], key[4][JIT_KW];
         const uint32_t alive = rowEval(stage, q, t * JIT_TILE_ROWS + q * 4, P, key, meas);
         jitAggregate(T, P, alive, key, meas, allowClaim, bypass, misses);
 #endif
@@ -730,9 +642,8 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
       }
       __syncthreads();
       for (uint32_t q = threadIdx.x; q * 4 < rows; q += JIT_THREADS) {
-        uint64_t meas[4];
         const uint32_t nvalid = rows - q * 4 < 4 ? rows - q * 4 : 4;
-#if JIT_DENSE && JIT_NMEAS > 1
+#if JIT_DENSE
         uint32_t dslot[JIT_NSLOT][4];
         bool fast[4], anySlow;
         uint64_t mv[JIT_NMEAS][4];
@@ -740,16 +651,9 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
 #pragma unroll
         for (int m = 0; m < JIT_NMEAS; m++) live[m] = 0xFu;
         if (rowEval(stages, q, done + q * 4, P, nvalid, fast, anySlow, JIT_DSLOT(dslot), mv[0], mr[0] JIT_MEAS_REST(mv, mr) JIT_LIVE_ARG(live)))
-          multiAggregateDense(touchedAddr, P, stages, q, done + q * 4, nvalid, repOff, fast, anySlow, dslot, mv, mr, live);
-        (void)meas;
-#elif JIT_DENSE
-        uint32_t dslot[4];
-        bool fast[4], anySlow;
-        uint32_t mraw[4];
-        if (rowEval(stages, q, done + q * 4, P, nvalid, fast, anySlow, dslot, meas, mraw))
-          jitAggregateDense(touchedAddr, tAcc, P, stages, q, done + q * 4, nvalid, repOff, fast, anySlow, dslot, meas, mraw);
+          jitAggregateDense(tableAddr, P, stages, q, done + q * 4, nvalid, repOff, fast, anySlow, dslot, mv, mr, live);
 #else
-        uint64_t key[4][JIT_KW];
+        uint64_t meas[4], key[4][JIT_KW];
         uint32_t alive = rowEval(stages, q, done + q * 4, P, key, meas);
         alive &= (1u << nvalid) - 1u;
         jitAggregate(T, P, alive, key, meas, true, false, misses);
@@ -762,40 +666,8 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
   if (JIT_HLL == 2) return;  // nothing CTA-private to fold: registers are updated in place
 #if JIT_DENSE == 2
   return;   // denseFoldKernel (batch_plan.cu) folds the shared array after the batch
-#elif JIT_DENSE && JIT_NMEAS > 1
-  multiFlush(P, denseSlots);
-  return;
 #elif JIT_DENSE
-  // fold the touched slots into the global table: the slot index decodes to the dimension values
-  for (uint32_t i = threadIdx.x; i < denseSlots; i += JIT_THREADS) {
-    unsigned long long accS = P.accNeutral;
-    if (JIT_DENSE_ACC == 4) {
-      // pieces -> integer -> double: only positive values were added, so 0 = no such row (adding the neutral element
-      // below is then a no-op); 2^-S is a power of two and the integer is exact below 2^53
-      const uint32_t *c = reinterpret_cast<const uint32_t *>(tKeys) + 3u * i;
-      const unsigned long long v = (unsigned long long)c[0] + ((unsigned long long)c[1] << 11) + ((unsigned long long)c[2] << 22);
-      if (v != 0) accS = (unsigned long long)__double_as_longlong(__ull2double_rn(v) * P.fxInv);
-    } else {
-      accS = denseSharedAcc()[i];
-    }
-    const unsigned long long accG = JIT_DENSE_ACC != 1 ? __ldcg(&tAcc[i]) : P.accNeutral;
-    if (JIT_DENSE_FLAGS ? !touched[i] : (accS == P.accNeutral && accG == P.accNeutral)) continue;
-    uint32_t rem = i % P.dRepStride, dvr[JIT_ND], vb = 0;   // (padding slots between copies are never reached)
-#pragma unroll
-    for (int k = JIT_ND - 1; k >= 0; k--) {
-      const uint32_t ix = rem / P.dStride[k];
-      rem -= ix * P.dStride[k];
-      const bool valid = ix != P.dCnt[k];
-      dvr[k] = valid ? (P.dLo[k] + ix) * P.dStep[k] : 0u;
-      vb |= (valid ? 1u : 0u) << k;
-    }
-    uint64_t key[JIT_KW];
-    densePack(dvr, vb, key);
-    const unsigned long long k = jitKeyOfRow(key);
-    // (the host does not wait for these kernels: when the table is at its growth threshold new groups are parked)
-    if (JIT_DENSE_ACC != 1) globalUpdate(P.G, (AggOp)JIT_AGG_OP, k, JIT_KW == 1 ? nullptr : key, accG, true);
-    globalUpdate(P.G, (AggOp)JIT_AGG_OP, k, JIT_KW == 1 ? nullptr : key, accS, true);
-  }
+  denseFlush(P, denseSlots);
   return;
 #endif
   // (the CTA's table is folded whatever the state of the global one: groups it cannot take right now are parked)

@@ -35,14 +35,14 @@ struct RleColumn {
   uint32_t length, startBit;
 };
 
-// One measure of a plan whose measure roots feed several states (JIT_NMEAS > 1): the state's group table, its CTA slices
-// and the constants the single-measure kernel takes from JitParams' own fields.
+// One measure of a direct-indexed plan (JIT_NMEAS of them): the group table and CTA slices of the state it feeds, and the
+// constants of its form.
 struct JitMeasure {
   DevTable G;
   unsigned long long *ctaAcc;
   unsigned long long measureIdentity, accNeutral;
-  double fxInv;
-  float fxScale;
+  double fxInv;                           // integer form (kMeasAcc 4): 2^-S
+  float fxScale;                          //                            2^S (a float sum's rows are added as integers x * 2^S)
   uint32_t pad;
 };
 
@@ -65,14 +65,11 @@ struct JitParams {
   uint32_t dStrideB[kJitMaxDenseDims];   // dStride in the unit the fast path addresses slots in (bytes for the integer form: x 12)
   uint32_t dTotal, dReps, dRepStride;     // slots of one copy; lane-private copies (power of two), dRepStride slots apart
   unsigned long long *gAcc;               // JIT_DENSE == 2: the state's global accumulator array (dTotal slots in use)
-  double fxInv;                           // JIT_DENSE_ACC == 4: 2^-S
-  float fxScale;                          //                     2^S (a float sum's rows are added as integers x * 2^S)
-  uint32_t fxPad;
   const DevJoin *join;                    // joined dimension tables (join.cuh), null without joins
   uint32_t resume;                        // 1: second launch of the same batch after the table grew (progress[] says where)
   uint32_t startCount;                    // row number of index position 0 when the batch has no base counts
   RleColumn rle[kJitMaxRle];              // run-length encoded columns decoded in place (see ldrle)
-  JitMeasure ms[kJitMaxMeasures];         // JIT_NMEAS > 1: measure m's state (unused by single-measure kernels)
+  JitMeasure ms[kJitMaxMeasures];         // direct-indexed CTA slots: measure m's state and form (ms[0]: the plan's own)
   // JIT_MDIMS (the measures differ in their dimensions): measure m's slot = sum_k index_k * mStride[m][k] (0 for a
   // dimension m does not have); lane-private copies of its slots, mRepStride[m] slots apart
   uint32_t mStride[kJitMaxMeasures][kJitMaxDenseDims];

@@ -46,8 +46,9 @@ struct DevInst {
   uint8_t rowOff, width, nullOff, pad;
 };
 
-// One measure root of a plan that feeds several states (DevPlan::nmeas > 1): what the single-measure plan of its state
-// decided (compilePlan + layoutStages on that plan), so that each measure takes the accumulation form it would take alone.
+// One measure root of a plan: what the single-measure plan of its state decided (compilePlan + layoutStages on that plan),
+// so that each measure of a plan that feeds several states (DevPlan::nmeas > 1) takes the accumulation form it would take
+// alone.  A single-measure plan describes its own measure in meas[0].
 struct DevMeasure {
   DevTable G;                    // the state's group table and CTA slices (filled just before the launch)
   unsigned long long *ctaAcc;
@@ -101,8 +102,7 @@ struct DevPlan {
   uint8_t denseGlobal;
   uint8_t denseGlobalReps;   // copies of the global slot array (power of two; CTA b uses copy b mod reps): spreads the L2 atomics
   uint8_t neutralSafe;     // no sequence of row values can bring a reached accumulator back to accNeutral (set by compilePlan)
-  uint8_t denseFx;         // float sum accumulated as exact integers (three 32-bit pieces per slot), see jitAnalyzeDense
-  int8_t fxMeasureInst;    // the measure instruction (a verbatim Float32 column with a zone map)
+  uint8_t denseFx;         // float sum accumulated as exact integers in the CTA's slots (three 32-bit pieces each), see jitAnalyzeDense
   int8_t fxShift;          // S: a row adds x * 2^S
   uint8_t numForeignTables, numForeignCols;
   uint8_t joinCol[kMaxForeignTables];       // main-table column matched with table t's primary key
