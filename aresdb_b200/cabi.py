@@ -352,11 +352,6 @@ _PLAN_SIGS = {
                             _VP, C.c_int],
     "AggStateReset": [_VP, _VP, C.c_int],
     "AggStateDestroy": [_VP, C.c_int],
-    "AggStateExportPart": [_VP, _VP, C.c_int, C.c_size_t, C.c_size_t, _VP, C.c_int],
-    "AggStateMergeParts": [_VP, _VP, C.c_int, C.c_size_t, C.c_int, C.c_size_t, C.c_size_t, _VP, C.c_int],
-    "AggStateExportPartToPeers": [_VP, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_size_t, C.c_int, C.c_size_t,
-                                  C.c_size_t, C.c_uint32, _VP, C.c_int],
-    "AggStateMergePartsWhenFlagged": [_VP, _VP, C.c_int, C.c_size_t, C.c_int, C.c_size_t, C.c_size_t, _VP, C.c_uint32, _VP, C.c_int],
     "AggStatesFinalize": [C.POINTER(C.c_void_p), C.c_int, C.POINTER(DimensionVector), C.POINTER(C.c_void_p), C.POINTER(C.c_int64), _VP,
                           C.c_int],
     "AggStatesExportPartsToPeers": [C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, C.c_int,

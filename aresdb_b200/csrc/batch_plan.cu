@@ -432,8 +432,8 @@ denseFoldKernel(unsigned long long *__restrict__ acc, DenseFold F, DevTable G) {
 // element: 8192 threads give every thread at most four elements, so a phase costs a few memory latencies, and the
 // phases are separated by the hardware cluster barrier (one CTA of 1024 threads would serialise those latencies).
 // The group count goes to a mapped pinned host word, so the
-// host's only interaction is one stream synchronise.  `ordered == 0` is the exchange form (AggStateExport /
-// AggStateExportPart): the claimed slots as they are, no sort, no merge.
+// host's only interaction is one stream synchronise.  `ordered == 0` is the exchange form of AggStateExport: the
+// claimed slots as they are, no sort, no merge.
 constexpr int kSmallFinalizeMax = kSmallSortMax;
 constexpr int kFinCtas = 8;                          // portable cluster maximum
 constexpr uint32_t kFinThreads = kFinCtas * 1024u;
@@ -483,8 +483,8 @@ __global__ void __cluster_dims__(kFinCtas, 1, 1) __launch_bounds__(1024, 1) fina
   const uint32_t n = G.counters[0];
   uint32_t status = SF_OK;
   if (G.counters[1]) status = SF_TABLE_OVERFLOW;
-  else if (G.counters[2] == 2u) status = SF_PEER_LATE;   // AggStateMergePartsWhenFlagged gave up waiting for a peer's part
-  else if (G.counters[2]) status = SF_PART_TRUNCATED;   // AggStateMergeParts met a part that did not hold all its rows
+  else if (G.counters[2] == 2u) status = SF_PEER_LATE;   // AggStatesMergeParts gave up waiting for a peer's flag
+  else if (G.counters[2]) status = SF_PART_TRUNCATED;   // AggStatesMergeParts met a part that did not hold all its rows
   else if (G.counters[3] || G.counters[4]) status = SF_UNSETTLED;   // stopped at the growth threshold / rows parked: the host settles first
   else if (n > (uint32_t)kSmallFinalizeMax) status = SF_TOO_MANY;
   else if (!A.ordered && n > (uint32_t)A.outCapacity) status = SF_OUTPUT_TOO_SMALL;
@@ -592,7 +592,7 @@ __global__ void __cluster_dims__(kFinCtas, 1, 1) __launch_bounds__(1024, 1) fina
 }
 
 // Exchange over peer memory, sending side: ONE kernel writes this rank's rows of every state as parts ([rows, status,
-// claimed | dimension block | measures], the layout of AggStateExportPart) into its own slot of its receive buffer —
+// claimed | dimension block | measures], AggStatesExportPartsToPeers' sub-part) into its own slot of its receive buffer —
 // cluster c (kFinCtas CTAs) exports state c into sub-part c —, copies each sub-part into the same place in every peer's
 // receive buffer with 16-byte stores over NVLink, and then stores `epoch` into state c's flag for this rank on every peer
 // (release, system scope) — export, all-gather and the "it has arrived" signal in one launch, no collective library and
@@ -2143,14 +2143,11 @@ static int64_t finalizeLarge(AggState *st, const DimensionVector &out, uint8_t *
   return g;
 }
 
-// Folds the exchange parts of numStates states (AggState(s)MergeParts / AggStateMergePartsWhenFlagged: `flags` != nullptr)
-// with one launch.
-static void mergeParts(AggState *const *sts, int numStates, const char *fn, const uint8_t *slots, int numParts, size_t slotStride,
-                       int capRows, const size_t *partOffset, const size_t *dimOffset, const size_t *valuesOffset, const uint32_t *flags,
+// Folds the exchange parts of numStates non-HLL states (AggStatesMergeParts; with `flags`, each state's CTAs first wait
+// for its senders' flags) with one launch.
+static void mergeParts(AggState *const *sts, int numStates, const uint8_t *slots, int numParts, size_t slotStride, int capRows,
+                       const size_t *partOffset, const size_t *dimOffset, const size_t *valuesOffset, const uint32_t *flags,
                        uint32_t epoch, cudaStream_t s) {
-  for (int k = 0; k < numStates; k++)
-    if (sts[k]->hll) throw EngineError(std::string(fn) + ": HLL states exchange through AggStateExport");
-  if (numParts <= 0) return;
   static thread_local MergePartsArgs M;
   memset(&M, 0, sizeof(M));
   for (int k = 0; k < numStates; k++) {
@@ -2165,14 +2162,14 @@ static void mergeParts(AggState *const *sts, int numStates, const char *fn, cons
   M.slots = slots; M.slotStride = slotStride; M.flags = flags; M.numParts = numParts; M.epoch = epoch;
   const int perState = smCount() * 2 / numStates;
   mergePartsKernel<<<dim3(perState > 0 ? perState : 1, numStates), 256, 0, s>>>(M);
-  checkLastError(fn);
+  checkLastError("mergeParts");
 }
 
 // Exchange-form export of numStates states into sub-parts of this rank's slot (peerSlots[myRank]) and, with peerFlags, the
 // copy into every peer's slot plus the arrival flags: one launch, asynchronous.
 static void exportPartsToPeers(AggState *const *sts, int numStates, uint8_t *const *peerSlots, uint32_t *const *peerFlags, int numPeers,
                                int myRank, const size_t *partBytes, int capRows, const size_t *partOffset, const size_t *dimOffset,
-                               const size_t *valuesOffset, uint32_t epoch, cudaStream_t s, const char *fn) {
+                               const size_t *valuesOffset, uint32_t epoch, cudaStream_t s) {
   static thread_local PeerExportArgs E;
   memset(&E, 0, sizeof(E));
   for (int r = 0; r < numPeers; r++) { E.peerSlot[r] = peerSlots[r]; E.peerFlag[r] = peerFlags ? peerFlags[r] : nullptr; }
@@ -2184,7 +2181,7 @@ static void exportPartsToPeers(AggState *const *sts, int numStates, uint8_t *con
   }
   E.numPeers = (uint32_t)numPeers; E.myRank = (uint32_t)myRank; E.epoch = epoch;
   exportToPeersKernel<<<kFinCtas * numStates, 1024, 0, s>>>(E);
-  checkLastError(fn);
+  checkLastError("exportToPeers");
 }
 
 // HLL state -> the reference's final outputs.  AggStateFinalize on such a state already yields the
@@ -2298,69 +2295,6 @@ CGoCallResHandle AggStateExport(void *state, DimensionVector outputKeys, uint8_t
   });
 }
 
-// Exchange form without host involvement (sharded queries): the claimed slots go to `part` = [uint32 rows, status,
-// claimed | ... | dimension block of capRows rows at dimOffset | measures at valuesOffset]; nothing is synchronised and
-// the row count stays on the device.  More rows than capRows (or than one CTA handles): status != 0, no rows.
-CGoCallResHandle AggStateExportPart(void *state, uint8_t *part, int capRows, size_t dimOffset, size_t valuesOffset,
-                                    void *cudaStream, int device) {
-  return guarded("AggStateExportPart", device, [&]() -> int64_t {
-    AggState *st = asState(state);
-    if (st->hll) throw EngineError("AggStateExportPart: HLL states exchange through AggStateExport");
-    if (capRows <= 0 || capRows > kSmallFinalizeMax) throw EngineError("AggStateExportPart: capRows must be in [1, 32768]");
-    SmallFinalizeArgs A = smallFinalizeArgs(st, capRows, part + dimOffset, part + valuesOffset, reinterpret_cast<uint32_t *>(part));
-    A.resultHost = st->resultHostDev + 4;   // host copy unused
-    launchSmallFinalize(&A, 1, (cudaStream_t)cudaStream, "AggStateExportPart");
-    return 0;
-  });
-}
-
-// Receiving side: folds `numParts` parts laid out `partStride` bytes apart (as all_gather leaves them) into `state` with
-// one launch; asynchronous.  A truncated part is reported by the next AggStateFinalize ("exchange part truncated").
-CGoCallResHandle AggStateMergeParts(void *state, const uint8_t *parts, int numParts, size_t partStride, int capRows,
-                                    size_t dimOffset, size_t valuesOffset, void *cudaStream, int device) {
-  return guarded("AggStateMergeParts", device, [&]() -> int64_t {
-    AggState *st = asState(state);
-    const size_t partOffset = 0;
-    mergeParts(&st, 1, "AggStateMergeParts", parts, numParts, partStride, capRows, &partOffset, &dimOffset, &valuesOffset, nullptr, 0u,
-               (cudaStream_t)cudaStream);
-    return 0;
-  });
-}
-
-// Exchange over peer memory (sharded queries on one NVLink / NVSwitch node).  `peerSlots[r]` = the address, in THIS
-// process, of this rank's part slot inside rank r's receive buffer; `peerFlags[r]` = the address of flags[myRank] on rank
-// r (the host maps the peers' buffers: CUDA IPC / fabric handles, e.g. torch symmetric memory).  One launch; asynchronous.
-CGoCallResHandle AggStateExportPartToPeers(void *state, uint8_t *const *peerSlots, uint32_t *const *peerFlags, int numPeers, int myRank,
-                                           size_t partBytes, int capRows, size_t dimOffset, size_t valuesOffset, uint32_t epoch,
-                                           void *cudaStream, int device) {
-  return guarded("AggStateExportPartToPeers", device, [&]() -> int64_t {
-    AggState *st = asState(state);
-    if (st->hll) throw EngineError("AggStateExportPartToPeers: HLL states exchange through AggStateExport");
-    if (capRows <= 0 || capRows > kSmallFinalizeMax) throw EngineError("AggStateExportPartToPeers: capRows must be in [1, 32768]");
-    if (numPeers <= 0 || numPeers > 16 || myRank < 0 || myRank >= numPeers) throw EngineError("AggStateExportPartToPeers: 1..16 peers");
-    if (partBytes % 16 != 0) throw EngineError("AggStateExportPartToPeers: partBytes must be a multiple of 16");
-    const size_t partOffset = 0;
-    exportPartsToPeers(&st, 1, peerSlots, peerFlags, numPeers, myRank, &partBytes, capRows, &partOffset, &dimOffset, &valuesOffset, epoch,
-                       (cudaStream_t)cudaStream, "AggStateExportPartToPeers");
-    return 0;
-  });
-}
-
-// Receiving side: as AggStateMergeParts, but the merge kernel itself waits (bounded) until every peer has stored `epoch`
-// into flags[peer].  A peer that does not arrive is reported by the next AggStateFinalize.
-CGoCallResHandle AggStateMergePartsWhenFlagged(void *state, const uint8_t *parts, int numParts, size_t partStride, int capRows,
-                                               size_t dimOffset, size_t valuesOffset, const uint32_t *flags, uint32_t epoch,
-                                               void *cudaStream, int device) {
-  return guarded("AggStateMergePartsWhenFlagged", device, [&]() -> int64_t {
-    if (flags == nullptr) throw EngineError("AggStateMergePartsWhenFlagged: flags is null");
-    AggState *st = asState(state);
-    const size_t partOffset = 0;
-    mergeParts(&st, 1, "AggStateMergePartsWhenFlagged", parts, numParts, partStride, capRows, &partOffset, &dimOffset, &valuesOffset,
-               flags, epoch, (cudaStream_t)cudaStream);
-    return 0;
-  });
-}
-
 // ---- several states per launch (the queries of one request) ----
 // The states of one call: 1..kMaxLaunchStates distinct, non-HLL AggStates.
 static void requestStates(void *const *states, int numStates, AggState **sts) {
@@ -2431,7 +2365,7 @@ CGoCallResHandle AggStatesExportPartsToPeers(void *const *states, int numStates,
     for (int r = 0; r < numPeers; r++)
       if ((r == myRank || peerFlags) && (!peerSlots[r] || (peerFlags && !peerFlags[r]))) throw EngineError("null peer slot or flag");
     exportPartsToPeers(sts, numStates, peerSlots, peerFlags, numPeers, myRank, partBytes, capRows, partOffset, dimOffset, valuesOffset,
-                       epoch, (cudaStream_t)cudaStream, "AggStatesExportPartsToPeers");
+                       epoch, (cudaStream_t)cudaStream);
     return 0;
   });
 }
@@ -2446,8 +2380,8 @@ CGoCallResHandle AggStatesMergeParts(void *const *states, int numStates, const u
     if (numParts < 1 || numParts > kMaxPeers) throw EngineError("numParts must be 1..16");
     size_t partBytes[kMaxLaunchStates];
     checkSlotLayout(sts, numStates, slotStride, capRows, partOffset, dimOffset, valuesOffset, partBytes);
-    mergeParts(sts, numStates, "AggStatesMergeParts", slots, numParts, slotStride, capRows, partOffset, dimOffset, valuesOffset, flags,
-               epoch, (cudaStream_t)cudaStream);
+    mergeParts(sts, numStates, slots, numParts, slotStride, capRows, partOffset, dimOffset, valuesOffset, flags, epoch,
+               (cudaStream_t)cudaStream);
     return 0;
   });
 }

@@ -1,10 +1,15 @@
-"""Multi-GPU execution of one aggregate query: table shards / archive batches are independent units
-(the reference processes them one after the other and only couples them through the carried result
-vectors, SURVEY.md §8e), so batch i goes to rank i mod N, every rank aggregates its batches into a
-private group table, and ONE exchange step merges the per-rank results: an all-gather of the compact
-(dimension block, measure vector) pairs over NCCL followed by a local re-aggregation on every rank
-with the aggregate's combine rule — what the reference's broker does with JSON results
+"""Multi-GPU execution of aggregate queries: table shards / archive batches are independent units (the reference
+processes them one after the other and only couples them through the carried result vectors, SURVEY.md §8e), so batch i
+goes to rank i mod N, every rank aggregates its batches into private group tables, and ONE exchange step merges the
+per-rank results with each aggregate's combine rule — what the reference's broker does with JSON results
 (broker/result_merge.go:80-105: sum/count add, min/max).  Results are identical on every rank.
+
+ShardedFusedRequest runs a rank's share of an AQL request; ShardedFusedQuery is a request of one query.  The exchange
+runs on the device: one export launch writes every query's rows as a fixed-capacity part and copies it into every peer's
+receive buffer over peer memory (or, where the ranks cannot map each other's buffers, one NCCL all-gather moves the
+parts), one merge launch folds the parts and one finalize launch completes every query.  Queries with more groups than a
+part holds and HLL queries take the exact-size protocol (exchange_exact).  ARESDB_B200_EXCHANGE chooses the transport:
+"peer" (the default), "fixed" (the all-gather) or "exact" (the exact-size protocol for every query).
 """
 from __future__ import annotations
 
@@ -15,7 +20,7 @@ import sys
 import numpy as np
 
 from . import cabi as A
-from .executor import MAX_LAUNCH_STATES, _ResultBuffers, dim_offsets, finalize_states, query_result
+from .executor import MAX_LAUNCH_STATES, dim_offsets, finalize_states, query_result
 from .query import AggQuery, QueryResult
 
 
@@ -26,136 +31,6 @@ _PART_HDR = 64          # a part's header (16 bytes used) in front of its dimens
 def assign_batches(num_batches: int, world: int, rank: int) -> list[int]:
     """Round-robin placement of batch ids."""
     return [b for b in range(num_batches) if b % world == rank]
-
-
-def pad_result(space, q: AggQuery, src: _ResultBuffers, groups: int, capacity: int) -> _ResultBuffers:
-    """Re-lays a result block out for `capacity` rows (all ranks must gather equal-sized tensors)."""
-    pad = _ResultBuffers(space, q, max(capacity, 1))
-    so, sn, widths, _ = dim_offsets(q.num_dims_per_width, src.capacity)
-    do, dn, _, _ = dim_offsets(q.num_dims_per_width, pad.capacity)
-    for p, w in enumerate(widths):
-        space.copy(pad.dims, do[p], src.dims, so[p], w * groups)
-        space.copy(pad.dims, dn[p], src.dims, sn[p], groups)
-    space.copy(pad.measures, 0, src.measures, 0, q.measure_bytes * groups)
-    return pad
-
-
-class ShardedFusedQuery:
-    """One rank's half of a sharded query on the B200 engine (torch.distributed / NCCL plumbing)."""
-
-    def __init__(self, lib, space, q: AggQuery, expected_groups: int = 0, merged_groups: int | None = None):
-        from .executor import FusedBatchExecutor
-        import torch.distributed as dist
-        self.dist = dist
-        self.world = dist.get_world_size() if dist.is_initialized() else 1
-        self.rank = dist.get_rank() if dist.is_initialized() else 0
-        self.lib, self.space, self.q = lib, space, q
-        self.local = FusedBatchExecutor(lib, space, q, expected_groups)
-        # the merged state sees every rank's groups: same table hint (and, for hll, the same table mode)
-        merged_groups = expected_groups if merged_groups is None else merged_groups
-        self.merged = FusedBatchExecutor(lib, space, q, merged_groups) if self.world > 1 else None
-        # Fixed-capacity exchange (queries that do not announce more groups than this): every rank sends
-        # [row count | dimension block | measures] for EXCHANGE_ROWS rows in ONE all-gather, so no count has to be agreed on
-        # first (one collective and one host sync less per query); a rank with more rows flags it in its header and
-        # every rank repeats the step with the exact-size protocol.
-        import os
-        self._fixed_cap = self.EXCHANGE_ROWS if (self.world > 1 and expected_groups <= self.EXCHANGE_ROWS and not q.is_hll
-                                                 and os.environ.get("ARESDB_B200_EXCHANGE", "fixed") != "exact") else 0
-        self._send = self._recv = None
-        self._peer, self._peer_ok = None, None   # exchange over peer memory: set up at the first exchange
-
-    def reset(self):
-        self.local.reset()
-
-    def process_batch(self, batch, stream=None):
-        self.local.process_batch(batch, stream)
-
-    EXCHANGE_ROWS = EXCHANGE_ROWS
-    _HDR = _PART_HDR
-
-    def _exchange_fixed(self):
-        """Device-only exchange: AggStateExportPart (one launch, the row count stays on the device) -> ONE all-gather of
-        the fixed parts -> AggStateMergeParts (one launch over all parts).  The host waits for nothing here; a rank with
-        more rows than a part holds marks its header and the merged state's finalize reports it (-> exact protocol)."""
-        import torch
-        q, sp, dist, lib = self.q, self.space, self.dist, self.lib
-        cap = self._fixed_cap
-        _, _, _, dim_bytes = dim_offsets(q.num_dims_per_width, cap)
-        dim_bytes = (dim_bytes + 15) // 16 * 16
-        part = (self._HDR + dim_bytes + q.measure_bytes * cap + 63) // 64 * 64
-        if self._send is None:
-            self._send = torch.zeros(part, dtype=torch.uint8, device=sp.dev)
-            self._recv = torch.empty(self.world * part, dtype=torch.uint8, device=sp.dev)
-        if self._peer is None and self._peer_ok is None:
-            self._setup_peers(part)
-        if self._peer is not None:
-            return self._exchange_peers(cap, dim_bytes)
-        lib.AggStateExportPart(self.local.state, self._send.data_ptr(), cap, self._HDR, self._HDR + dim_bytes, sp.stream, sp.device)
-        dist.all_gather_into_tensor(self._recv, self._send)
-        self.merged.reset()
-        lib.AggStateMergeParts(self.merged.state, self._recv.data_ptr(), self.world, part, cap, self._HDR, self._HDR + dim_bytes,
-                               sp.stream, sp.device)
-        return self.world * cap
-
-    _FLAGS = 256   # two parities x 16 ranks x uint32, in front of the two receive buffers
-
-    def _setup_peers(self, part: int):
-        self._peer = setup_peer_buffers(self.dist, self.space, self.world, self._FLAGS + 2 * self.world * part)
-        self._peer_ok = self._peer is not None
-        if self._peer is not None:
-            self._peer["part"] = part
-
-    def _exchange_peers(self, cap: int, dim_bytes: int):
-        """AggStateExportPartToPeers (ONE launch: export + copy of the part into every peer's receive buffer over NVLink +
-        the arrival flags) -> AggStateMergePartsWhenFlagged (the merge kernel waits for the peers' flags itself).  No
-        collective call, no host wait; receive buffers alternate by epoch parity (a rank is at most one exchange ahead)."""
-        import ctypes as C
-        pe, sp, lib, w, r = self._peer, self.space, self.lib, self.world, self.rank
-        pe["epoch"] += 1
-        epoch, par, part = pe["epoch"], pe["epoch"] & 1, pe["part"]
-        base = self._FLAGS + par * w * part
-        slots = (C.c_void_p * w)(*[pe["ptrs"][p] + base + r * part for p in range(w)])
-        flags = (C.c_void_p * w)(*[pe["ptrs"][p] + par * 64 + r * 4 for p in range(w)])
-        lib.AggStateExportPartToPeers(self.local.state, slots, flags, w, r, part, cap, self._HDR, self._HDR + dim_bytes, epoch,
-                                      sp.stream, sp.device)
-        self.merged.reset()
-        lib.AggStateMergePartsWhenFlagged(self.merged.state, pe["ptrs"][r] + base, w, part, cap, self._HDR, self._HDR + dim_bytes,
-                                          pe["ptrs"][r] + par * 64, epoch, sp.stream, sp.device)
-        return w * cap
-
-    def _exchange(self):
-        if self._fixed_cap:
-            return self._exchange_fixed()
-        return self._exchange_exact()
-
-    def _exchange_exact(self):
-        rows, self._keep = exchange_exact(self.dist, self.world, self.rank, self.local, self.merged)
-        return rows
-
-    def finalize(self):
-        """(groups, result buffers) of the WHOLE query, identical on every rank."""
-        if self.world == 1:
-            return self.local.finalize_into()
-        if self._fixed_cap:
-            self._exchange_fixed()
-            try:
-                return self.merged.finalize_into()
-            except A.AresError as e:
-                if "exchange part truncated" not in str(e):
-                    raise
-        return self.merged.finalize_into(self._exchange_exact())
-
-    def finalize_hll(self):
-        """hll queries: the HLLResult of the WHOLE query, identical on every rank."""
-        if self.world == 1:
-            return self.local.hll_result()
-        self._exchange()
-        return self.merged.hll_result()
-
-    def close(self):
-        self.local.close()
-        if self.merged:
-            self.merged.close()
 
 
 def setup_peer_buffers(dist, space, world: int, nbytes: int):
@@ -234,7 +109,7 @@ class ShardedFusedRequest:
     FusedRequestExecutor, so queries that share dimensions, time filter and joins share the scan on every rank.  finalize() exchanges
     every non-HLL query that announces at most EXCHANGE_ROWS groups in ONE export launch (the rank's slot holds one
     sub-part per query; over peer memory when every rank can map every other's receive buffer, else one NCCL all-gather
-    — ARESDB_B200_EXCHANGE as for ShardedFusedQuery), folds them with ONE merge launch and finalizes them with ONE
+    — see ARESDB_B200_EXCHANGE in the module docstring), folds them with ONE merge launch and finalizes them with ONE
     AggStatesFinalize.  HLL queries, queries that announce more groups and queries whose sub-part was truncated take the
     exact-size protocol (exchange_exact)."""
 
@@ -306,11 +181,16 @@ class ShardedFusedRequest:
 
     def finalize(self) -> list:
         """One result per query, in request order, identical on every rank: a QueryResult, or an HLLResult for HLL queries."""
+        return [r if q.is_hll else query_result(q, *r) for q, r in zip(self.queries, self._finalize())]
+
+    def _finalize(self) -> list:
+        """The exchange and finalize step: per query, in request order, (groups, _ResultBuffers) with the result left in
+        device memory, or the HLLResult of an HLL query."""
         if self.world == 1:
             return self._results(self.local.executors, {})
         if self._merged_dirty:
-            for m in self.merged:
-                m.reset()
+            for i in self.fixed:   # (exchange_exact resets the states it merges into)
+                self.merged[i].reset()
         self._merged_dirty = True
         done, exact = {}, [i for i in range(len(self.queries)) if i not in self.fixed]
         if self.fixed:
@@ -338,13 +218,38 @@ class ShardedFusedRequest:
             elif isinstance(done[i], Exception):
                 raise done[i]
             else:
-                out.append(query_result(q, *done[i]))
+                out.append(done[i])
         return out
 
     def close(self):
         self.local.close()
         for m in self.merged or []:
             m.close()
+
+
+class ShardedFusedQuery:
+    """One rank's half of a sharded query: a ShardedFusedRequest of this one query, whose results stay in device memory."""
+
+    def __init__(self, lib, space, q: AggQuery, expected_groups: int = 0):
+        self.q = q
+        self.request = ShardedFusedRequest(lib, space, [q], expected_groups)
+
+    def process_batch(self, batch, stream=None):
+        self.request.process_batch(batch, stream)
+
+    def reset(self):
+        self.request.reset()
+
+    def finalize(self):
+        """(groups, _ResultBuffers) of the WHOLE query, identical on every rank."""
+        return self.request._finalize()[0]
+
+    def finalize_hll(self):
+        """HLL queries: the HLLResult of the WHOLE query, identical on every rank."""
+        return self.request._finalize()[0]
+
+    def close(self):
+        self.request.close()
 
 
 # ---- host-side mirror (gloo / CPU): same protocol on QueryResults, used by the CPU test-suite ------

@@ -223,36 +223,9 @@ CGoCallResHandle AggStateFinalize(void *state, DimensionVector outputKeys, uint8
 CGoCallResHandle AggStateExport(void *state, DimensionVector outputKeys, uint8_t *outputValues,
                                 void *cudaStream, int device);
 
-/* The exchange step of a sharded query without host involvement.  AggStateExportPart writes this state's rows as ONE
- * fixed-capacity part — [uint32 rows, uint32 status, uint32 claimed, pad | DimensionVector block of capRows rows at
- * dimOffset | measures at valuesOffset] — with one launch and no synchronisation (the row count stays on the device);
- * the parts of all ranks are all-gathered; AggStateMergeParts folds every gathered part into the receiving state with one
- * launch, reading the counts from the part headers.  capRows <= 32768.  A state with more rows marks its part
- * (status != 0, no rows) and the receiver's next AggStateFinalize fails with "exchange part truncated": repeat the step
- * with AggStateGroupCount / AggStateExport / AggStateMerge (exact sizes).  Not for AGGR_HLL states. */
-CGoCallResHandle AggStateExportPart(void *state, uint8_t *part, int capRows, size_t dimOffset, size_t valuesOffset,
-                                    void *cudaStream, int device);
-CGoCallResHandle AggStateMergeParts(void *state, const uint8_t *parts, int numParts, size_t partStride, int capRows,
-                                    size_t dimOffset, size_t valuesOffset, void *cudaStream, int device);
-
-/* The same exchange over PEER MEMORY (one NVLink / NVSwitch node), without a collective library: the host maps every
- * rank's receive buffer into every process (CUDA IPC / fabric handles — torch symmetric memory does it) and hands over
- * peerSlots[r] = the address of THIS rank's part slot inside rank r's receive buffer and peerFlags[r] = the address of
- * flags[myRank] on rank r.  AggStateExportPartToPeers is ONE launch: it writes the part into the local slot, copies it
- * into every peer's slot with 16-byte stores over NVLink and then stores `epoch` into the flag on every peer (release,
- * system scope).  AggStateMergePartsWhenFlagged is AggStateMergeParts whose kernel first waits (bounded: ~2 s, then the
- * next AggStateFinalize fails) until all numParts flags have reached `epoch`.  Use two receive buffers alternately and a
- * growing epoch: a rank can be at most one exchange ahead of its peers.  numPeers <= 16, partBytes % 16 == 0. */
-CGoCallResHandle AggStateExportPartToPeers(void *state, uint8_t *const *peerSlots, uint32_t *const *peerFlags, int numPeers, int myRank,
-                                           size_t partBytes, int capRows, size_t dimOffset, size_t valuesOffset, uint32_t epoch,
-                                           void *cudaStream, int device);
-CGoCallResHandle AggStateMergePartsWhenFlagged(void *state, const uint8_t *parts, int numParts, size_t partStride, int capRows,
-                                               size_t dimOffset, size_t valuesOffset, const uint32_t *flags, uint32_t epoch,
-                                               void *cudaStream, int device);
-
 /* The queries of one request, several states per launch (1..16 distinct states; AGGR_HLL states are refused — they keep
  * the exact protocol).  Every call below rejects null arrays, a numStates outside 1..16, a state given twice and an HLL
- * state with an error.
+ * state with an error.  A single query is a request of one state (one-element arrays).
  *
  * AggStatesFinalize: AggStateFinalize of states[k] into (outputKeys[k], outputValues[k]); groups[k] = its group count.
  * States that announce at most 32768 groups are finalized by ONE launch (one cluster each) and ONE synchronise; the
@@ -261,20 +234,31 @@ CGoCallResHandle AggStateMergePartsWhenFlagged(void *state, const uint8_t *parts
  * truncated") the others are still finalized: its groups[k] is -1 and the error lists every failed state as a line
  * "state k: <message>".  outputKeys[k] must have states[k]'s NumDimsPerDimWidth.
  *
+ * The exchange step of a sharded request, without host involvement: every rank exports its states as fixed-capacity
+ * parts, the parts of all ranks reach every rank, and every rank folds them into its receiving states, whose next
+ * AggStatesFinalize completes the request.  Nothing is synchronised and the row counts stay on the device.
+ *
  * AggStatesExportPartsToPeers: ONE launch exports every state into its sub-part of this rank's slot — sub-part k at
- * partOffset[k] inside the slot, laid out as AggStateExportPart's part (16-byte header [rows, status, claimed, pad],
- * dimension block of capRows rows at dimOffset[k], measures at valuesOffset[k], both relative to the sub-part) — in
- * peerSlots[myRank], copies every sub-part into peerSlots[r] of every peer r, and then stores `epoch` into state k's flag
- * for this rank on every peer: peerFlags[r] + 16 * k, where peerFlags[r] = the address of flags[0][myRank] on rank r (a
- * rank's flags are uint32 flags[state][16 ranks]).  peerFlags == NULL: the local export only (peerSlots[myRank]; the
- * slots then travel by a collective all-gather).  capRows in [1, 32768]; slotBytes and every offset are multiples of 16,
- * and each sub-part lies inside the slot without overlapping another; numPeers in 1..16, 0 <= myRank < numPeers.
+ * partOffset[k] inside the slot: a 16-byte header [uint32 rows, uint32 status, uint32 claimed, pad], the DimensionVector
+ * block of capRows rows at dimOffset[k] and the measures at valuesOffset[k], both relative to the sub-part — in
+ * peerSlots[myRank], copies every sub-part into peerSlots[r] of every peer r with 16-byte stores, and then stores `epoch`
+ * into state k's flag for this rank on every peer (release, system scope): peerFlags[r] + 16 * k, where peerFlags[r] =
+ * the address of flags[0][myRank] on rank r (a rank's flags are uint32 flags[state][16 ranks]).  peerSlots[r] is the
+ * address of THIS rank's slot inside rank r's receive buffer: the host maps every rank's receive buffer into every
+ * process (peer memory on one NVLink / NVSwitch node: CUDA IPC / fabric handles — torch symmetric memory does it).
+ * peerFlags == NULL: the local export only (peerSlots[myRank]; the slots then travel by a collective all-gather).
+ * capRows in [1, 32768]; slotBytes and every offset are multiples of 16, and each sub-part lies inside the slot without
+ * overlapping another; numPeers in 1..16, 0 <= myRank < numPeers.  A state with more rows than capRows marks its
+ * sub-part (status != 0, no rows): the receiving state's next finalize fails with "exchange part truncated", and that
+ * state's step is repeated with AggStateGroupCount / AggStateExport / AggStateMerge (exact sizes).
  *
  * AggStatesMergeParts: ONE launch folds, for every state k, sub-part k of each of the numParts slots (slot p at
- * slots + p * slotStride, as an all-gather or the peers' exports leave them) into states[k].  flags != NULL: the CTAs of
- * state k first wait (bounded, as AggStateMergePartsWhenFlagged) until flags[16 * k + p] has reached `epoch` for every
- * p < numParts; a state never waits for another state's flags.  A truncated sub-part or a late peer is reported by that
- * state's next finalize only.  Use two flag blocks and receive buffers alternately by epoch parity, with a growing epoch.
+ * slots + p * slotStride, as an all-gather or the peers' exports leave them) into states[k], reading the row counts from
+ * the sub-part headers.  flags != NULL: the CTAs of state k first wait until flags[16 * k + p] has reached `epoch` for
+ * every p < numParts; a state never waits for another state's flags.  The wait is bounded (~2 s): a peer that does not
+ * arrive makes that state's next finalize fail ("did not arrive") instead of hanging the GPU.  A truncated sub-part or a
+ * late peer is reported by that state's next finalize only.  Use two flag blocks and receive buffers alternately by
+ * epoch parity, with a growing epoch: a rank can be at most one exchange ahead of its peers.
  * All three are asynchronous except AggStatesFinalize, which synchronises. */
 CGoCallResHandle AggStatesFinalize(void *const *states, int numStates, const DimensionVector *outputKeys, uint8_t *const *outputValues,
                                    int64_t *groups, void *cudaStream, int device);

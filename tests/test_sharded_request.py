@@ -241,11 +241,12 @@ def _same_results(qs, got, exp, ctx):
 @pytest.mark.gpu
 def test_request_without_process_group_equals_request_executor():
     """world == 1: ShardedFusedRequest gives FusedRequestExecutor's results (HLLResults for HLL queries), for plain batches
-    and for a shard scan (live batches behind the cutoff filter, then the archive days)."""
+    and for a shard scan (live batches behind the cutoff filter, then the archive days); so does a ShardedFusedQuery per
+    query of the request."""
     import harness as H
     from aresdb_b200 import aql, archive
-    from aresdb_b200.executor import FusedRequestExecutor
-    from aresdb_b200.sharding import ShardedFusedRequest
+    from aresdb_b200.executor import FusedRequestExecutor, query_result
+    from aresdb_b200.sharding import ShardedFusedQuery, ShardedFusedRequest
     eng = H.get_backend("b200")
     qs = _request()
     batches = [T.upload(eng, hb, 0, synth.zone_map(hb)) for hb in (synth.generate_batch(d, 20000, num_cities=30) for d in range(3))]
@@ -255,8 +256,15 @@ def test_request_without_process_group_equals_request_executor():
         ref.process_batch(b)
     exp = [ex.hll_result() if q.is_hll else r for q, ex, r in zip(qs, ref.executors, ref.results())]
     _same_results(qs, req.finalize(), exp, "batches")
-    req.close()
-    ref.close()
+    # one ShardedFusedQuery per query (what bench.py runs): results left in device memory, HLLResults for HLL queries
+    one = [ShardedFusedQuery(eng.lib, eng.space, q) for q in qs]
+    for b in batches:
+        for s in one:
+            s.process_batch(b)
+    got = [s.finalize_hll() if q.is_hll else query_result(q, *s.finalize()) for q, s in zip(qs, one)]
+    _same_results(qs, got, exp, "one query")
+    for x in one + [req, ref]:
+        x.close()
     # archive.scan_shard
     table = aql.Table("trips", [aql.Column(n, t) for n, t in zip(synth.COLUMN_NAMES, synth.COLUMN_TYPES)])
     day0, cutoff = synth.BASE_TS // 86400, synth.BASE_TS + 3 * 86400
