@@ -12,8 +12,9 @@
 //   * surviving rows are aggregated into a CTA-private table (or direct-indexed slots when the
 //     zone map bounds every dimension), which is flushed into the L2-resident global group table
 //     when the CTA retires; rows that do not fit it go to the global table directly.
-// Here: the plan's device form (compilePlan), its inputs made stageable (executePlan: run-length
-// columns, unaligned parts), the stage layout (layoutStages) and the launch / resume protocol.
+// Here: the plan's device form (compilePlan), its inputs made stageable (describeInputs / materialiseInputs:
+// run-length columns, unaligned parts), the stage layout (layoutStages), the kernels a batch runs (scheduleBatch) and
+// the launch / resume protocol (executePlan).
 // The global table lives in an AggState across batches.  AggStateFinalize compacts it, hashes
 // each group's packed dimension row with the reference's murmur3, sorts the g groups by hash,
 // merges equal hashes and writes the reference's output layout — the observable result of the
@@ -1104,7 +1105,7 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P, Agg
 // ---------------------------------------------------------------------------------------
 // archive batches: run-length encoded (mode-3) columns that the kernel does not decode from their runs
 // are expanded once per batch into plain mode-2 scratch columns (one value + one validity bit per
-// index position), see prepareInputs.
+// index position), see describeInputs.
 // ---------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 expandRleKernel(InputDesc d, const uint32_t *__restrict__ baseCounts, uint32_t startCount, uint32_t n, int width, bool direct,
@@ -1164,7 +1165,7 @@ static bool stagesBaseCounts(const DevPlan &P) {
 }
 
 // What a laid-out single-measure plan decided for its measure (denseFx: it takes the exact-integer form), as the kernel's
-// per-measure code takes it: for the plan itself, or for a state's measure in a shared plan (planShared).
+// per-measure code takes it: for the plan itself, or for a state's measure in a shared plan (scheduleStates).
 static void describeMeasure(const DevPlan &Q, DevMeasure &M) {
   M.aggOp = Q.aggOp; M.measWidth = Q.measWidth; M.skipCount = Q.skipCount; M.neutralSafe = Q.neutralSafe;
   M.denseFx = Q.denseFx; M.fxShift = Q.fxShift; M.measureIdentity = Q.measureIdentity; M.accNeutral = Q.accNeutral;
@@ -1197,7 +1198,7 @@ static bool memberSlots(DevPlan &P, size_t avail) {
 
 // Decides the tile size, the stage layout, the TMA ring depth and the shared table size.  The shared table gets what the
 // workload needs first (a table that overflows sends rows to contended L2 atomics, tools/microbench/agg_microbench.cu),
-// the ring takes the rest.  Staged parts must start on a 16-byte boundary (executePlan copies those that do not).
+// the ring takes the rest.  Staged parts must start on a 16-byte boundary (materialiseInputs copies those that do not).
 // A single-measure plan describes its measure in meas[0].
 static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
   const bool stageBc = stagesBaseCounts(P);
@@ -1239,7 +1240,7 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
         // (several measures: one 128-byte aligned region of accumulators each)
         const size_t need = 128 + n * stageBytesFor(tr) + (P.nmeas > 1 && !P.memberDims ? 128 * P.nmeas : 0);
         if (need >= (size_t)kSmemBudget) continue;
-        if (P.memberDims) {   // (only with several measures: planShared)
+        if (P.memberDims) {   // (only with several measures: scheduleStates)
           if (memberSlots(P, (size_t)kSmemBudget - need)) {
             tileRows = tr; stages = n; slots = 16;
             for (int m = 0; m < P.nmeas; m++) slots = P.meas[m].slots > slots ? P.meas[m].slots : slots;
@@ -1445,7 +1446,12 @@ static void ensureRoom(AggState *st, uint64_t bound, cudaStream_t s) {
   st->occUpper += bound;
 }
 
-// Makes every input of the plan readable by the kernel as it is (before layoutStages).
+// An RLE column whose count vector IS the batch's base counts: its run p holds index position p.
+static bool countsAreBaseCounts(const InputDesc &in, const BatchPlan &bp) {
+  return bp.BaseCounts != nullptr && reinterpret_cast<const uint32_t *>(in.base) == bp.BaseCounts;
+}
+
+// Describes every input of the plan as the kernel will read it (before layoutStages), without device work.
 // Archive batches: run-length encoded (mode 3) columns.
 //  * the column whose count vector IS the batch's base counts has one value per index position: it is read like an
 //    uncompressed column (values / null bitmap of its runs), no copy;
@@ -1453,24 +1459,17 @@ static void ensureRoom(AggState *st, uint64_t bound, cudaStream_t s) {
 //    the tile loop (jit_kernel_head.cuh ldrle) with a per-tile run hint computed by executePlan — HBM sees the runs, not
 //    the rows;
 //  * the others (and 8- / 16-byte ones, which the kernel reads row by row) are expanded once per batch into mode-2
-//    scratch columns (one value + one validity bit per index position).
-// Staged parts (values and null bitmaps of 1- to 4-byte columns, the base counts) are fetched by the TMA engine, which
-// needs a 16-byte aligned source: a part that is not aligned is copied once, byte for byte (same bit offset).
-// `scratch` == nullptr (AresJitDryRun, no device memory): descriptors are rewritten as if, nothing is allocated, copied
-// or launched — the kernel text does not depend on addresses.
-static void prepareInputs(DevPlan &P, const BatchPlan &bp, cudaStream_t s, std::vector<std::unique_ptr<Scratch>> *scratch) {
+//    scratch columns (one value + one validity bit per index position): described here, made by materialiseInputs.
+// The layout and the kernel text depend on these descriptors and never on the addresses materialiseInputs sets:
+// layoutStages (with jitAnalyzeDense) does not read DevColumn::in.base, and reads DevPlan::baseCounts only to test it
+// for null.  That is what lets a batch's launches be scheduled before any of them runs.
+static void describeInputs(DevPlan &P, const BatchPlan &bp) {
   const uint32_t n = P.numRows;
-  auto alloc = [&](size_t bytes) -> uint8_t * {
-    if (scratch == nullptr) return nullptr;
-    scratch->emplace_back(new Scratch(bytes, s));
-    return scratch->back()->as<uint8_t>();
-  };
   int nrle = 0;
   for (int c = 0; c < P.ncols; c++) {
     DevColumn &col = P.cols[c];
     if (!col.used || col.in.mode != 3) continue;
-    const bool direct = bp.BaseCounts != nullptr && reinterpret_cast<const uint32_t *>(col.in.base) == bp.BaseCounts;
-    if (direct && col.in.length >= n) {   // run number == index position
+    if (countsAreBaseCounts(col.in, bp) && col.in.length >= n) {   // run number == index position
       col.in.mode = 2;
       continue;
     }
@@ -1479,24 +1478,40 @@ static void prepareInputs(DevPlan &P, const BatchPlan &bp, cudaStream_t s, std::
       nrle++;
       continue;
     }
-    const size_t nullBytes = ((size_t)(n + 31) / 32 * 4 + 16 + 63) / 64 * 64;
-    const size_t valueBytes = (col.width ? (size_t)n * col.width : (size_t)(n + 31) / 32 * 4) + 64;
-    uint8_t *buf = alloc(nullBytes + valueBytes);
-    if (buf != nullptr) {
-      int blocks = divUp((int64_t)(n + 31) / 32, 8);
-      if (blocks > smCount() * 16) blocks = smCount() * 16;
-      expandRleKernel<<<blocks, 256, 0, s>>>(col.in, bp.BaseCounts, bp.StartCount, n, col.width, direct, buf + nullBytes,
-                                             reinterpret_cast<uint32_t *>(buf));
-      checkLastError("expandRle");
-    }
-    col.in.base = buf;
+    col.expand = 1;
+    col.in.base = nullptr;
     col.in.nullsOff = 0;
-    col.in.valuesOff = (uint32_t)nullBytes;
+    col.in.valuesOff = (uint32_t)(((size_t)(n + 31) / 32 * 4 + 16 + 63) / 64 * 64);   // the null bitmap comes first
     col.in.length = n;
     col.in.mode = 2;
     col.in.startBit = 0;
   }
-  if (scratch == nullptr) return;
+}
+
+// Makes the inputs describeInputs described readable by the kernel of a laid-out plan: the expanded columns are made
+// from the batch's RLE columns, and the first-class ones get their run hints.  Staged parts (values and null bitmaps of
+// 1- to 4-byte columns, the base counts) are fetched by the TMA engine, which needs a 16-byte aligned source: a part that
+// is not aligned is copied once, byte for byte (same bit offset).
+static void materialiseInputs(DevPlan &P, const BatchPlan &bp, cudaStream_t s, std::vector<std::unique_ptr<Scratch>> &scratch) {
+  const uint32_t n = P.numRows;
+  auto alloc = [&](size_t bytes) {
+    scratch.emplace_back(new Scratch(bytes, s));
+    return scratch.back()->as<uint8_t>();
+  };
+  for (int c = 0; c < P.ncols; c++) {
+    DevColumn &col = P.cols[c];
+    if (!col.expand) continue;
+    const InputDesc runs = makeColumnDesc(bp.Columns[c], /*allowWide=*/true);
+    const size_t nullBytes = col.in.valuesOff;
+    const size_t valueBytes = (col.width ? (size_t)n * col.width : (size_t)(n + 31) / 32 * 4) + 64;
+    uint8_t *buf = alloc(nullBytes + valueBytes);
+    int blocks = divUp((int64_t)(n + 31) / 32, 8);
+    if (blocks > smCount() * 16) blocks = smCount() * 16;
+    expandRleKernel<<<blocks, 256, 0, s>>>(runs, bp.BaseCounts, bp.StartCount, n, col.width, countsAreBaseCounts(runs, bp),
+                                           buf + nullBytes, reinterpret_cast<uint32_t *>(buf));
+    checkLastError("expandRle");
+    col.in.base = buf;
+  }
   auto misaligned = [](const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; };
   for (int c = 0; c < P.ncols; c++) {
     DevColumn &col = P.cols[c];
@@ -1518,6 +1533,16 @@ static void prepareInputs(DevPlan &P, const BatchPlan &bp, cudaStream_t s, std::
     uint8_t *buf = alloc(((size_t)n + 1) * 4);
     ARES_CUDA(cudaMemcpyAsync(buf, P.baseCounts, ((size_t)n + 1) * 4, cudaMemcpyDefault, s));
     P.baseCounts = reinterpret_cast<const uint32_t *>(buf);
+  }
+  for (int c = 0; c < P.ncols; c++) {   // per-tile run hints of the first-class RLE columns (layoutStages sized the tiles)
+    DevColumn &col = P.cols[c];
+    if (!col.rle) continue;
+    const uint32_t entries = (P.numRows + P.tileRows - 1) / P.tileRows + 2;
+    uint32_t *hints = reinterpret_cast<uint32_t *>(alloc(sizeof(uint32_t) * entries));
+    rleTileRunsKernel<<<divUp(entries, 256), 256, 0, s>>>(reinterpret_cast<const uint32_t *>(col.in.base), col.in.length, bp.BaseCounts,
+                                                         bp.StartCount, P.numRows, P.tileRows, entries, hints);
+    checkLastError("rleTileRuns");
+    col.tileRun = hints;
   }
 }
 
@@ -1543,20 +1568,6 @@ static void uploadJoin(DevPlan &P, const BatchPlan &bp, cudaStream_t s, std::uni
   }
 }
 
-// Per-tile run hints of the first-class RLE columns (after layoutStages: the tile size is known).
-static void rleTileHints(DevPlan &P, const BatchPlan &bp, cudaStream_t s, std::vector<std::unique_ptr<Scratch>> &scratch) {
-  for (int c = 0; c < P.ncols; c++) {
-    DevColumn &col = P.cols[c];
-    if (!col.rle) continue;
-    const uint32_t entries = (P.numRows + P.tileRows - 1) / P.tileRows + 2;
-    scratch.emplace_back(new Scratch(sizeof(uint32_t) * entries, s));
-    rleTileRunsKernel<<<divUp(entries, 256), 256, 0, s>>>(reinterpret_cast<const uint32_t *>(col.in.base), col.in.length, bp.BaseCounts,
-                                                         bp.StartCount, P.numRows, P.tileRows, entries, scratch.back()->as<uint32_t>());
-    checkLastError("rleTileRuns");
-    col.tileRun = scratch.back()->as<uint32_t>();
-  }
-}
-
 // one CTA per SM, or per full tile when there are fewer; a batch without a full tile is the tail of one CTA
 static int launchGrid(const DevPlan &P) {
   int grid = smCount() < kMaxGridCtas ? smCount() : kMaxGridCtas;
@@ -1564,32 +1575,28 @@ static int launchGrid(const DevPlan &P) {
   return grid;
 }
 
-// Launches the kernel of a laid-out plan whose measures feed sts[0..n).  Direct-indexed kernels are not waited for (see
-// "growth of the group table"): what their flush may insert (the CTA slots; the global slot array's fold) is reserved in
-// every state's table up front, and their out-of-range rows park.  Hash-table kernels are checked by the caller.
-static void launchPlan(DevPlan &P, AggState *const *sts, int n, cudaStream_t s) {
-  for (int k = 0; k < n; k++) {
-    if (P.denseNd != 0) ensureRoom(sts[k], (uint64_t)(P.memberDims ? P.meas[k].total : P.denseTotal), s);
-    P.meas[k].G = sts[k]->table;      // (after a possible growth: the slices live in the table's allocation)
-    P.meas[k].ctaAcc = sts[k]->ctaAcc;
-  }
-  P.ctaAcc = sts[0]->ctaAcc;
-  jitLaunch(P, sts[0]->table, 128 + (size_t)P.tableBytes + (size_t)P.stageBytes * P.numStages, launchGrid(P), s);
-}
+// One kernel launch of a batch (see scheduleBatch): the states it feeds, the plan it runs — the batch's plan, a dimension
+// set's or one state's (measurePlan) — and that plan's device form, laid out for this batch.
+struct Launch {
+  AggState *sts[kJitMaxMeasures];
+  int n;
+  bool set;                // the plan of a dimension set (member dimensions)
+  const BatchPlan *plan;
+  DevPlan *P;
+};
 
-static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
-  if (bp.NumRows == 0) return;
-  if (bp.NumRows > 0x7FFFFFFFu) throw EngineError("a batch holds at most 2^31-1 rows");
-  static thread_local DevPlan P;  // ~3 KB
-  compilePlan(st, bp, P);
+// Runs one launch of a batch: materialises its inputs, launches its kernel and, for a hash-table kernel, checks it and
+// resumes it when the table's growth stopped it.
+static void executePlan(const Launch &L, cudaStream_t s) {
+  DevPlan &P = *L.P;
+  AggState *st = L.sts[0];
   P.resume = 0;
   std::vector<std::unique_ptr<Scratch>> scratch;   // expanded / realigned columns, run hints: released in stream order
-  prepareInputs(P, bp, s, &scratch);
+  materialiseInputs(P, *L.plan, s, scratch);
   std::unique_ptr<Scratch> joinMem;
-  uploadJoin(P, bp, s, joinMem);
-  layoutStages(P, st->spec.ExpectedGroups);
-  rleTileHints(P, bp, s, scratch);
-  // hash-table kernels are checked after the launch and resumed when they stopped
+  uploadJoin(P, *L.plan, s, joinMem);
+  // hash-table kernels are checked after the launch and resumed when they stopped (a kernel that feeds several states is
+  // direct-indexed)
   const bool resumable = P.denseNd == 0 && !st->hllDense;
   if (P.denseGlobal) {
     if (!st->denseAcc) {   // first use: 16 MB of accumulators at the neutral element (denseFoldKernel leaves them so)
@@ -1600,7 +1607,15 @@ static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
     P.denseAcc = st->denseAcc;
   }
   for (;;) {
-    launchPlan(P, &st, 1, s);
+    // Direct-indexed kernels are not waited for (see "growth of the group table"): what their flush may insert (the CTA
+    // slots; the global slot array's fold) is reserved in every state's table up front, and their out-of-range rows park.
+    for (int k = 0; k < L.n; k++) {
+      if (P.denseNd != 0) ensureRoom(L.sts[k], (uint64_t)(P.memberDims ? P.meas[k].total : P.denseTotal), s);
+      P.meas[k].G = L.sts[k]->table;      // (after a possible growth: the slices live in the table's allocation)
+      P.meas[k].ctaAcc = L.sts[k]->ctaAcc;
+    }
+    P.ctaAcc = st->ctaAcc;
+    jitLaunch(P, st->table, 128 + (size_t)P.tableBytes + (size_t)P.stageBytes * P.numStages, launchGrid(P), s);
     if (P.denseGlobal) {
       DenseFold F;
       memset(&F, 0, sizeof(F));
@@ -1644,7 +1659,7 @@ static void executePlan(AggState *st, const BatchPlan &bp, cudaStream_t s) {
 }
 
 // ---------------------------------------------------------------------------------------
-// several measures over one scan (ExecuteBatchPlanMulti)
+// the launches of a batch: one plan, or several measures over one scan (ExecuteBatchPlanMulti)
 // ---------------------------------------------------------------------------------------
 static bool hasSink(const BatchPlan &bp, int sink) {
   for (int i = 0; i < bp.NumInsts && i < ARES_MAX_PLAN_INSTS; i++)
@@ -1655,7 +1670,6 @@ static bool hasSink(const BatchPlan &bp, int sink) {
 // States that may share a plan: the same reduce mode, no HLL, and the same dimension layout unless the plan gives each
 // state its own dimensions (member dimensions, checked by compilePlan).
 static void checkSharedStates(AggState *const *sts, int n, const BatchPlan &bp) {
-  if (n < 1 || n > kJitMaxMeasures) throw EngineError("numStates must be 1.." + std::to_string(kJitMaxMeasures));
   const bool memberDims = hasSink(bp, PLAN_SINK_MEMBER_DIMENSION);
   for (int k = 0; k < n; k++) {
     if (sts[k]->hll) throw EngineError("AGGR_HLL states cannot share a plan");
@@ -1664,13 +1678,6 @@ static void checkSharedStates(AggState *const *sts, int n, const BatchPlan &bp) 
     if (sts[k]->spec.ReduceMode != sts[0]->spec.ReduceMode) throw EngineError("states differ in ReduceMode");
   }
 }
-
-// Single-measure plans of the states of a shared plan (BatchPlan has no default constructor: raw storage).
-struct MeasurePlans {
-  std::vector<unsigned char> mem;
-  void resize(int n) { mem.resize(sizeof(BatchPlan) * n); }
-  BatchPlan &operator[](int k) { return reinterpret_cast<BatchPlan *>(mem.data())[k]; }
-};
 
 // The plan of the states in `set` (bit k = state k): every instruction except the other states' measure, member filter
 // and member dimension roots and the sub-expressions only they consume.  The kept states are renumbered in order; their
@@ -1731,97 +1738,109 @@ static std::vector<uint32_t> dimensionSets(int n, const BatchPlan &bp) {
   return sets;
 }
 
-// Compiles the shared plan into P and decides its form for this batch.  true: one kernel feeds every state — each
-// measure's own single-measure plan takes the CTA's direct-indexed slots, and all of them fit a CTA together (P is then
-// laid out, without device work when `scratch` is null).  false: the caller runs the states' own plans, or (member
-// dimensions) the plans of the states' dimension sets.  `subs` holds the single-measure plans either way.
-static bool planShared(AggState *const *sts, int n, const BatchPlan &bp, DevPlan &P, MeasurePlans &subs,
-                       cudaStream_t s, std::vector<std::unique_ptr<Scratch>> *scratch) {
-  compilePlan(sts[0], bp, P, sts, n);
-  subs.resize(n);
-  for (int k = 0; k < n; k++) measurePlan(bp, 1u << k, subs[k]);
-  if (bp.NumRows == 0) return false;
-  static thread_local DevPlan Q;
+// The launches of one batch in launch order (a state is fed by exactly one), and the plans and device plans they use:
+// the batch's plan, each state's own plan at most twice (in the batch and in its dimension set), one per dimension set.
+// Thread-local, reused by every batch of the thread (BatchPlan has no default constructor: raw storage).
+struct Schedule {
+  static constexpr int kMaxPlans = 3 * kJitMaxMeasures;
+  int count, nplans, ndev;
+  Launch launch[kJitMaxMeasures];
+  DevPlan dev[kMaxPlans + 1];
+  alignas(BatchPlan) unsigned char planMem[kMaxPlans][sizeof(BatchPlan)];
+  BatchPlan &newPlan() { assert(nplans < kMaxPlans); return *reinterpret_cast<BatchPlan *>(planMem[nplans++]); }
+  DevPlan &newDevPlan() { assert(ndev <= kMaxPlans); return dev[ndev++]; }
+  void add(AggState *const *sts, int n, const BatchPlan &plan, DevPlan &P, bool set) {
+    Launch &L = launch[count++];
+    std::copy(sts, sts + n, L.sts);
+    L.n = n; L.set = set; L.plan = &plan; L.P = &P;
+  }
+};
+
+// Schedules states sts[0..n) over `bp`, compiled for them into P (with `multi` when n > 1).  One state runs P.  Several
+// share one kernel when each state's own plan (measurePlan) takes the CTA's direct-indexed slots and all of them fit a
+// CTA together: P is then laid out with every measure in the form its own plan takes.  Otherwise, with member
+// dimensions, each set of states with the same dimensions (dimensionSets order) is scheduled the same way, so a batch
+// never runs more kernels than states; without, each state runs its own plan, in state order.
+static void scheduleStates(Schedule &S, AggState *const *sts, int n, const BatchPlan &bp, DevPlan &P, bool set) {
+  if (n == 1) {
+    describeInputs(P, bp);
+    layoutStages(P, sts[0]->spec.ExpectedGroups);
+    S.add(sts, 1, bp, P, set);
+    return;
+  }
+  BatchPlan *own[kJitMaxMeasures];
+  DevPlan *Q[kJitMaxMeasures];
   bool shared = true;
   bool skipCount = true;
+  uint32_t expected = 0;
   for (int k = 0; k < n; k++) {
-    compilePlan(sts[k], subs[k], Q);
-    prepareInputs(Q, subs[k], nullptr, nullptr);
-    layoutStages(Q, sts[k]->spec.ExpectedGroups);
-    shared = shared && Q.denseNd != 0 && !Q.denseGlobal;
-    describeMeasure(Q, P.meas[k]);
-    skipCount = skipCount && Q.skipCount;
+    own[k] = &S.newPlan();
+    measurePlan(bp, 1u << k, *own[k]);
+    Q[k] = &S.newDevPlan();
+    compilePlan(sts[k], *own[k], *Q[k]);
+    describeInputs(*Q[k], *own[k]);
+    layoutStages(*Q[k], sts[k]->spec.ExpectedGroups);
+    shared = shared && Q[k]->denseNd != 0 && !Q[k]->denseGlobal;
+    describeMeasure(*Q[k], P.meas[k]);
+    skipCount = skipCount && Q[k]->skipCount;
+    expected = sts[k]->spec.ExpectedGroups > expected ? sts[k]->spec.ExpectedGroups : expected;
     // member dimensions: every state packs its rows with the kernel's one key form (JIT_KW / JIT_ROW_BYTES)
     if (P.memberDims && (sts[k]->keyMode != sts[0]->keyMode ||
                          (sts[k]->keyMode == KEY_HASHED && sts[k]->rowLayout.rowBytes != sts[0]->rowLayout.rowBytes)))
       shared = false;
   }
-  if (!shared) return false;
-  P.nmeas = (uint8_t)n;
-  P.skipCount = skipCount;   // base counts are staged when some measure counts run lengths
-  static thread_local DevPlan D;
-  D = P;   // the layout decision first, on a copy: prepareInputs rewrites the column descriptors
-  prepareInputs(D, bp, s, nullptr);
-  uint32_t expected = 0;
-  for (int k = 0; k < n; k++) expected = sts[k]->spec.ExpectedGroups > expected ? sts[k]->spec.ExpectedGroups : expected;
-  if (layoutStages(D, expected) == 0) return false;
-  if (scratch == nullptr) { P = D; return true; }
-  prepareInputs(P, bp, s, scratch);
-  layoutStages(P, expected);
-  return P.denseNd != 0;
-}
-
-// The plan one state runs for ExecuteBatchPlanMulti with numStates == 1: `bp` itself, or — when it has member filters
-// or member dimensions, checked as in a shared plan — `bp` with them turned into filters and dimensions (stored in `one`).
-static const BatchPlan &singleStatePlan(AggState *const *sts, const BatchPlan &bp, MeasurePlans &one) {
-  if (!hasSink(bp, PLAN_SINK_MEASURE_FILTER) && !hasSink(bp, PLAN_SINK_MEMBER_DIMENSION)) return bp;
-  static thread_local DevPlan Q;
-  compilePlan(sts[0], bp, Q, sts, 1);
-  one.resize(1);
-  measurePlan(bp, 1u, one[0]);
-  return one[0];
-}
-
-// The states of `set` and the plan of their dimension set (member dimensions become their dimensions).
-static int setStates(AggState *const *sts, uint32_t set, const BatchPlan &bp, AggState **out, BatchPlan &plan) {
-  int m = 0;
-  for (int k = 0; k < kJitMaxMeasures; k++)
-    if ((set >> k) & 1u) out[m++] = sts[k];
-  measurePlan(bp, set, plan);
-  return m;
-}
-
-static void executePlanMulti(AggState *const *sts, int n, const BatchPlan &bp, cudaStream_t s) {
-  checkSharedStates(sts, n, bp);
-  if (n == 1) {
-    MeasurePlans one;
-    executePlan(sts[0], singleStatePlan(sts, bp, one), s);
-    return;
-  }
-  if (bp.NumRows > 0x7FFFFFFFu) throw EngineError("a batch holds at most 2^31-1 rows");
-  static thread_local DevPlan P;
-  MeasurePlans subs;
-  std::vector<std::unique_ptr<Scratch>> scratch;
-  if (!planShared(sts, n, bp, P, subs, s, &scratch)) {
-    if (P.memberDims) {   // one pass per dimension set, each deciding its own form (never more kernels than states)
-      const std::vector<uint32_t> sets = dimensionSets(n, bp);
-      MeasurePlans plans;
-      plans.resize((int)sets.size());
-      for (size_t j = 0; j < sets.size(); j++) {
-        AggState *ss[kJitMaxMeasures];
-        const int m = setStates(sts, sets[j], bp, ss, plans[(int)j]);
-        executePlanMulti(ss, m, plans[(int)j], s);
-      }
+  if (shared) {
+    P.nmeas = (uint8_t)n;
+    P.skipCount = skipCount;   // base counts are staged when some measure counts run lengths
+    describeInputs(P, bp);
+    if (layoutStages(P, expected) != 0) {
+      S.add(sts, n, bp, P, set);
       return;
     }
-    for (int k = 0; k < n; k++) executePlan(sts[k], subs[k], s);
+  }
+  if (!P.memberDims) {
+    for (int k = 0; k < n; k++) S.add(&sts[k], 1, *own[k], *Q[k], false);
     return;
   }
-  P.resume = 0;
-  std::unique_ptr<Scratch> joinMem;
-  uploadJoin(P, bp, s, joinMem);
-  rleTileHints(P, bp, s, scratch);
-  launchPlan(P, sts, n, s);
+  for (uint32_t mask : dimensionSets(n, bp)) {
+    AggState *ss[kJitMaxMeasures];
+    int m = 0;
+    for (int k = 0; k < n; k++)
+      if ((mask >> k) & 1u) ss[m++] = sts[k];
+    BatchPlan &plan = S.newPlan();
+    measurePlan(bp, mask, plan);
+    DevPlan &Q1 = S.newDevPlan();
+    compilePlan(ss[0], plan, Q1, ss, m);
+    scheduleStates(S, ss, m, plan, Q1, true);
+  }
+}
+
+// The one decision of which kernels a batch runs, for ExecuteBatchPlan (multi = false, n = 1), ExecuteBatchPlanMulti
+// and the dry runs: validates the plan and schedules its launches (none for an empty batch) without device work;
+// executePlan materialises each launch's inputs when it runs.  One state of ExecuteBatchPlanMulti runs the plan with its
+// member filters and dimensions turned into plain ones.
+static const Schedule &scheduleBatch(AggState *const *sts, int n, const BatchPlan &bp, bool multi) {
+  static thread_local Schedule S;
+  S.count = S.nplans = S.ndev = 0;
+  if (multi) checkSharedStates(sts, n, bp);
+  if (bp.NumRows > 0x7FFFFFFFu) throw EngineError("a batch holds at most 2^31-1 rows");
+  DevPlan &P = S.newDevPlan();
+  compilePlan(sts[0], bp, P, multi ? sts : nullptr, multi ? n : 0);
+  if (bp.NumRows == 0) return S;
+  const BatchPlan *plan = &bp;
+  if (n == 1 && multi && (hasSink(bp, PLAN_SINK_MEASURE_FILTER) || hasSink(bp, PLAN_SINK_MEMBER_DIMENSION))) {
+    BatchPlan &one = S.newPlan();
+    measurePlan(bp, 1u, one);
+    compilePlan(sts[0], one, P);
+    plan = &one;
+  }
+  scheduleStates(S, sts, n, *plan, P, false);
+  return S;
+}
+
+static void executeBatch(AggState *const *sts, int n, const BatchPlan &bp, bool multi, cudaStream_t s) {
+  const Schedule &S = scheduleBatch(sts, n, bp, multi);
+  for (int i = 0; i < S.count; i++) executePlan(S.launch[i], s);
 }
 
 static void mergeRows(AggState *st, const DimensionVector &in, const uint8_t *values, int length, cudaStream_t s) {
@@ -2225,6 +2244,41 @@ static int64_t finalizeHLL(AggState *st, uint8_t **dimValuesPtr, uint8_t **hllVe
   return dims;
 }
 
+// The dry runs: schedules `plan` for AggStates described by `specs`, without device memory.  A schedule of one launch for
+// all of them is generated and NVRTC-compiled: returns the cubin size, and *sourceOut (optional) gets a malloc'd copy of
+// the kernel's shape-specific source.  Any other schedule is reported as an error that says which kernels run instead.
+static size_t dryRun(const AggSpec *specs, int n, const BatchPlan &plan, bool multi, char **sourceOut) {
+  AggState st[kJitMaxMeasures] = {}, *sts[kJitMaxMeasures];
+  for (int k = 0; k < n; k++) {
+    describeState(&st[k], specs[k]);
+    st[k].capacity = st[k].hllDense ? kHllDenseSlots : 0;
+    sts[k] = &st[k];
+  }
+  const Schedule &S = scheduleBatch(sts, n, plan, multi);
+  if (S.count == 0) throw EngineError("the batch is empty: no kernel runs");
+  if (S.count == 1 && S.launch[0].n == n) {
+    std::string src;
+    const size_t size = jitCompileOnly(*S.launch[0].P, &src);
+    if (sourceOut) *sourceOut = strdup(src.c_str());
+    return size;
+  }
+  bool perState = true, perSet = true;
+  std::string groups;
+  for (int i = 0; i < S.count; i++) {
+    const Launch &L = S.launch[i];
+    const bool direct = L.P->denseNd != 0;
+    perState = perState && L.n == 1 && !(L.set && direct);
+    perSet = perSet && L.set && direct;
+    groups += i ? ", {" : "{";
+    for (int j = 0; j < L.n; j++) groups += (j ? ", " : "") + std::to_string(std::find(sts, sts + n, L.sts[j]) - sts);
+    groups += direct ? "} direct-indexed" : "}";
+  }
+  if (perState) throw EngineError("this plan and zone map run one kernel per state (no shared direct-indexed form)");
+  if (perSet)
+    throw EngineError("this plan and zone map run one kernel per dimension set (" + std::to_string(S.count) + " sets, each direct-indexed)");
+  throw EngineError("this plan and zone map run " + std::to_string(S.count) + " kernels, one kernel per group of states: " + groups);
+}
+
 }  // namespace aresb
 
 using namespace aresb;
@@ -2245,7 +2299,8 @@ CGoCallResHandle AggStateCreate(AggSpec spec, void *cudaStream, int device) {
 CGoCallResHandle ExecuteBatchPlan(void *state, const BatchPlan *plan, void *cudaStream, int device) {
   return guarded("ExecuteBatchPlan", device, [&]() -> int64_t {
     if (!plan) throw EngineError("null plan");
-    executePlan(asState(state), *plan, (cudaStream_t)cudaStream);
+    AggState *st = asState(state);
+    executeBatch(&st, 1, *plan, false, (cudaStream_t)cudaStream);
     return 0;
   });
 }
@@ -2256,7 +2311,7 @@ CGoCallResHandle ExecuteBatchPlanMulti(void *const *states, int numStates, const
     if (!states || numStates < 1 || numStates > kJitMaxMeasures) throw EngineError("numStates must be 1.." + std::to_string(kJitMaxMeasures));
     AggState *sts[kJitMaxMeasures];
     for (int k = 0; k < numStates; k++) sts[k] = asState(states[k]);
-    executePlanMulti(sts, numStates, *plan, (cudaStream_t)cudaStream);
+    executeBatch(sts, numStates, *plan, true, (cudaStream_t)cudaStream);
     return 0;
   });
 }
@@ -2411,82 +2466,26 @@ CGoCallResHandle AggStateReset(void *state, void *cudaStream, int device) {
   });
 }
 
-// Additive diagnostics, usable without a GPU: generates + NVRTC-compiles the specialised kernel of
-// (spec, plan) and returns the cubin size in res; *sourceOut (optional) gets a malloc'd copy of the
-// generated shape-specific source.
+// Additive diagnostics, usable without a GPU: the kernel ExecuteBatchPlan runs for (spec, plan), generated and compiled;
+// res = cubin size.
 CGoCallResHandle AresJitDryRun(AggSpec spec, const BatchPlan *plan, char **sourceOut) {
   CGoCallResHandle h = {nullptr, nullptr};
   try {
-    AggState st;
-    memset(&st.table, 0, sizeof(st.table));
-    describeState(&st, spec);
-    st.capacity = st.hllDense ? kHllDenseSlots : 0;
-    static thread_local DevPlan P;
-    compilePlan(&st, *plan, P);
-    prepareInputs(P, *plan, nullptr, nullptr);
-    layoutStages(P, spec.ExpectedGroups);
-    std::string src;
-    size_t n = jitCompileOnly(P, &src);
-    if (sourceOut) *sourceOut = strdup(src.c_str());
-    h.res = reinterpret_cast<void *>(n);
+    h.res = reinterpret_cast<void *>(dryRun(&spec, 1, *plan, false, sourceOut));
   } catch (const std::exception &e) {
     h.pStrErr = strdup((std::string("AresJitDryRun: ") + e.what()).c_str());
   }
   return h;
 }
 
-// Additive diagnostics, usable without a GPU: the kernel of a plan whose measure roots feed numSpecs states (the shared
-// form of ExecuteBatchPlanMulti for this batch's zone map), generated and compiled; res = cubin size.  A plan that would
-// run as one kernel per state (no shared form for this batch) is reported as an error.
+// Additive diagnostics, usable without a GPU: the kernel of a plan whose measure roots feed numSpecs states, when
+// ExecuteBatchPlanMulti runs it as one kernel for all of them for this batch's zone map; res = cubin size.  Any other
+// schedule (one kernel per state, per dimension set, or a mix) is reported as an error.
 CGoCallResHandle AresJitDryRunMulti(const AggSpec *specs, int numSpecs, const BatchPlan *plan, char **sourceOut) {
   CGoCallResHandle h = {nullptr, nullptr};
   try {
     if (!specs || !plan || numSpecs < 1 || numSpecs > kJitMaxMeasures) throw EngineError("numSpecs must be 1.." + std::to_string(kJitMaxMeasures));
-    std::vector<AggState> st(numSpecs);
-    AggState *sts[kJitMaxMeasures];
-    for (int k = 0; k < numSpecs; k++) {
-      memset(&st[k].table, 0, sizeof(st[k].table));
-      describeState(&st[k], specs[k]);
-      st[k].capacity = 0;
-      sts[k] = &st[k];
-    }
-    checkSharedStates(sts, numSpecs, *plan);
-    static thread_local DevPlan P;
-    MeasurePlans subs;
-    if (numSpecs == 1) {
-      const BatchPlan &one = singleStatePlan(sts, *plan, subs);
-      compilePlan(sts[0], one, P);
-      prepareInputs(P, one, nullptr, nullptr);
-      layoutStages(P, specs[0].ExpectedGroups);
-    } else if (!planShared(sts, numSpecs, *plan, P, subs, nullptr, nullptr)) {
-      if (P.memberDims) {   // the per-set form: does every dimension set run as one direct-indexed kernel?
-        const std::vector<uint32_t> sets = dimensionSets(numSpecs, *plan);
-        std::unique_ptr<DevPlan> Q(new DevPlan);
-        MeasurePlans plans, more;
-        plans.resize((int)sets.size());
-        bool direct = true;
-        for (size_t j = 0; j < sets.size() && direct; j++) {
-          AggState *ss[kJitMaxMeasures];
-          const int m = setStates(sts, sets[j], *plan, ss, plans[(int)j]);
-          if (m > 1) {
-            direct = planShared(ss, m, plans[(int)j], *Q, more, nullptr, nullptr);
-          } else {
-            compilePlan(ss[0], plans[(int)j], *Q);
-            prepareInputs(*Q, plans[(int)j], nullptr, nullptr);
-            layoutStages(*Q, ss[0]->spec.ExpectedGroups);
-            direct = Q->denseNd != 0;
-          }
-        }
-        if (direct)
-          throw EngineError("this plan and zone map run one kernel per dimension set (" + std::to_string(sets.size()) +
-                            " sets, each direct-indexed)");
-      }
-      throw EngineError("this plan and zone map run one kernel per state (no shared direct-indexed form)");
-    }
-    std::string src;
-    size_t n = jitCompileOnly(P, &src);
-    if (sourceOut) *sourceOut = strdup(src.c_str());
-    h.res = reinterpret_cast<void *>(n);
+    h.res = reinterpret_cast<void *>(dryRun(specs, numSpecs, *plan, true, sourceOut));
   } catch (const std::exception &e) {
     h.pStrErr = strdup((std::string("AresJitDryRunMulti: ") + e.what()).c_str());
   }

@@ -30,7 +30,8 @@ struct DevColumn {
   uint32_t rangeLo, rangeHi;  // zone map of the batch (BatchPlan.Ranges): valid values lie in [rangeLo, rangeHi]
   uint8_t rangeKnown;
   uint8_t rle;             // run-length encoded (mode 3) column decoded in the kernel from its runs — never expanded, never staged
-  uint8_t pad[2];
+  uint8_t expand;          // run-length encoded column read as a plain copy: `in` describes the copy (base set when it is made)
+  uint8_t pad[1];
   const uint32_t *tileRun; // rle: run that holds the first index position of every tile (+ one entry for the last position)
 };
 

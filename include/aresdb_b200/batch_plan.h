@@ -193,8 +193,9 @@ CGoCallResHandle ExecuteBatchPlan(void *state, const BatchPlan *plan, void *cuda
  *      sized by its own slot count) fit a CTA together, and the states agree in key form (rows of at most 8 bytes, or
  *      rows of the same length); a row's index in every union dimension is computed once, and each state's slot is
  *      derived from the indexes of its own dimensions;
- *   2. otherwise one ExecuteBatchPlanMulti per set of states with identical dimensions (the plan of that set: its
- *      measure and member filter roots, its dimensions as PLAN_SINK_DIMENSION roots), each deciding its form as above;
+ *   2. otherwise each set of states with identical dimensions runs the plan of that set (its measure and member
+ *      filter roots, its dimensions as PLAN_SINK_DIMENSION roots), the sets in the order of their first state, each
+ *      taking its form as above: one kernel for the set, or one kernel per state of the set;
  *   3. when no such set takes a direct-indexed form, that is one kernel per state.
  * Every state gets exactly the result it gets alone.  A caller builds the union from the states' dimension
  * expressions, compared structurally together with their output type: each state's dimensions must appear in the

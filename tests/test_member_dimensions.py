@@ -11,6 +11,7 @@ equals the same query run alone on FusedBatchExecutor, and the launches per batc
 import ctypes as C
 import hashlib
 import json
+import re
 from pathlib import Path
 
 import pytest
@@ -55,6 +56,18 @@ def sets_panel():
     h2 = [E.floor(TS, E.Lit(7200)), CITY]
     return [AggQuery(f, [HOUR, CITY], Measure("sum", FARE)), AggQuery(f, [HOUR, CITY], Measure("count")),
             AggQuery(f, h2, Measure("count")), AggQuery(f, h2, Measure("max", CITY))]
+
+
+def mixed_panel():
+    """Two members by hour x city and two by status: without a zone-map range for status only the first set takes a
+    direct-indexed kernel, and the members by status run their own kernels."""
+    f = T.queries()["cfg3_sum"].filters
+    return [AggQuery(f, [HOUR, CITY], Measure("sum", FARE)), AggQuery(f, [HOUR, CITY], Measure("count")),
+            AggQuery(f, [STATUS], Measure("count")), AggQuery(f, [STATUS], Measure("max", CITY))]
+
+
+def without_status(ranges):
+    return {c: r for c, r in ranges.items() if c != synth.COL_STATUS}
 
 
 def filtered_panel(reduce_mode=A.ARES_REDUCE_SORT):
@@ -173,7 +186,8 @@ def test_packing_of_groups_into_passes():
 def test_dry_runs_choose_the_form():
     """The cfg3 panel: one kernel with the day's zone map (each member keeps the form it takes alone); two hour x city
     members and two two-hour x city members over 300 cities: one kernel per dimension set; no zone map: one kernel per
-    state.  With 300 cities the cfg3 panel itself still fits one kernel: only one member groups by hour x city."""
+    state; a set that fits next to a set without a zone map: the set's kernel and one kernel per other member.  With 300
+    cities the cfg3 panel itself still fits one kernel: only one member groups by hour x city."""
     lib = A.load_engine()
     qs = panel()
     size, src = S.dry_run_multi(lib, qs, MF.plan_of(qs, rows=125_000_000, ranges=S.CFG3_RANGES)[0])
@@ -191,6 +205,9 @@ def test_dry_runs_choose_the_form():
         assert "#define JIT_NMEAS 2" in S.dry_run_multi(lib, plan_qs, MF.plan_of(plan_qs, rows=125_000_000, ranges=WIDE)[0])[1]
     with pytest.raises(A.AresError, match="one kernel per state"):
         S.dry_run_multi(lib, qs, MF.plan_of(qs, rows=125_000_000)[0])
+    mq = mixed_panel()
+    with pytest.raises(A.AresError, match=r"run 3 kernels, one kernel per group of states: \{0, 1\} direct-indexed, \{2\}, \{3\}$"):
+        S.dry_run_multi(lib, mq, MF.plan_of(mq, rows=125_000_000, ranges=without_status(S.CFG3_RANGES))[0])
 
 
 def test_one_state_with_member_dimensions_is_its_own_plan(monkeypatch):
@@ -292,7 +309,8 @@ def test_forms_and_member_filters_equal_solo_runs(request_of, reduce_mode):
 @pytest.mark.gpu
 def test_launches_follow_the_form():
     """(1, 1) when the pass fits a CTA; one launch per dimension set when only the sets fit (300 cities); nothing when
-    the zone map contradicts every member."""
+    the zone map contradicts every member; a direct-indexed set next to members without a zone map: the kernels the dry
+    run reports for each batch's plan."""
     import harness as H
     eng = H.get_backend("b200")
     batches = []
@@ -305,6 +323,14 @@ def test_launches_follow_the_form():
     gone = [AggQuery([big], [HOUR], Measure("count")), AggQuery([big, E.eq(STATUS, E.Lit(1))], [CITY], Measure("sum", FARE))]
     per_batch, got = _run(eng, gone, batches)
     assert per_batch == [(0, 0), (0, 0)] and all(r.groups == 0 for r in got), per_batch
+    mixed, reported = mixed_panel(), []
+    for b in batches:
+        b.ranges = without_status(b.ranges)
+        with pytest.raises(A.AresError) as e:
+            S.dry_run_multi(eng.lib, mixed, MF.plan_of(mixed, rows=b.num_rows, ranges=b.ranges)[0])
+        reported.append(int(re.search(r"run (\d+) kernels", str(e.value)).group(1)))
+    per_batch, _ = _run(eng, mixed, batches)
+    assert reported == [3, 3] and per_batch == [(k, 1) for k in reported], (reported, per_batch)
 
 
 @pytest.mark.gpu
