@@ -815,7 +815,7 @@ static AggState *asState(void *p) {
   return static_cast<AggState *>(p);
 }
 
-static uint8_t operandClassOf(const PlanOperand &o, const BatchPlan &bp, const std::vector<uint8_t> &stackClasses) {
+static uint8_t operandClassOf(const PlanOperand &o, const BatchPlan &bp) {
   switch (o.Kind) {
     case PLAN_OPERAND_COLUMN: {
       if (o.Column >= bp.NumColumns) throw EngineError("plan operand references a column outside BatchPlan.Columns");
@@ -833,9 +833,6 @@ static uint8_t operandClassOf(const PlanOperand &o, const BatchPlan &bp, const s
       if (o.ConstType == ConstInt) return VC_I32;
       if (o.ConstType == ConstFloat) return VC_F32;
       throw EngineError("Unsupported constant type in plan");
-    case PLAN_OPERAND_STACK:
-      if (stackClasses.empty()) throw EngineError("plan pops an empty evaluation stack");
-      return stackClasses.back();
     case PLAN_OPERAND_FOREIGN: {
       if (o.Column >= bp.NumForeignColumns) throw EngineError("plan operand references a column outside BatchPlan.ForeignColumns");
       switch (bp.ForeignColumns[o.Column].Column.DataType) {
@@ -922,7 +919,7 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P, Agg
     P.foreignTableOf[k] = (uint8_t)t;
   }
   const DimLayout &RL = st->rowLayout;
-  std::vector<uint8_t> stack;
+  std::vector<int> stack;   // the instructions whose pushed values are on the evaluation stack
   std::vector<bool> dimSeen(RL.numDims, false);
   bool measureSeen = false;
   std::vector<bool> stateFed(nmulti, false);
@@ -930,19 +927,27 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P, Agg
   int firstMemberFilter = -1, firstDimOrMeasure = -1, firstMeasure = -1;
   bool plainDims = false;
   std::vector<int> memberDimsOf(nmulti, 0);   // member dimension roots of each state so far
+  int nmagic = 0;
   for (int i = 0; i < bp.NumInsts; i++) {
     const PlanInst &pi = bp.Insts[i];
     DevInst &I = P.insts[i];
     if (pi.NumOperands != 1 && pi.NumOperands != 2) throw EngineError("plan instruction must have 1 or 2 operands");
     I.nops = pi.NumOperands; I.fn = pi.Functor; I.sink = pi.Sink; I.sinkArg = pi.SinkArg;
-    // operand classes (rhs popped first when both come from the stack)
-    uint8_t bcls = VC_NONE, acls;
-    if (pi.NumOperands == 2) {
-      if (pi.B.Kind == PLAN_OPERAND_STACK) { bcls = operandClassOf(pi.B, bp, stack); stack.pop_back(); }
-    }
-    acls = operandClassOf(pi.A, bp, stack);
-    if (pi.A.Kind == PLAN_OPERAND_STACK) stack.pop_back();
-    if (pi.NumOperands == 2 && pi.B.Kind != PLAN_OPERAND_STACK) bcls = operandClassOf(pi.B, bp, stack);
+    // Each stack operand is linked to the instruction that pushed its value (the right operand pops first when both come
+    // from the stack); a stack operand's class is its producer's sink class.  The later passes follow the links and
+    // resolve operand a, then b: resolving a stack operand has no side effect (the generator emits no load for it and
+    // takes no JitParams::consts slot), so the order they read the links in changes neither the kernel text nor its
+    // parameters.
+    auto pop = [&]() -> int {
+      if (stack.empty()) throw EngineError("plan pops an empty evaluation stack");
+      const int j = stack.back();
+      stack.pop_back();
+      return j;
+    };
+    I.bsrc = (int8_t)(pi.NumOperands == 2 && pi.B.Kind == PLAN_OPERAND_STACK ? pop() : -1);
+    I.asrc = (int8_t)(pi.A.Kind == PLAN_OPERAND_STACK ? pop() : -1);
+    const uint8_t acls = I.asrc >= 0 ? P.insts[I.asrc].oclass : operandClassOf(pi.A, bp);
+    const uint8_t bcls = pi.NumOperands != 2 ? (uint8_t)VC_NONE : I.bsrc >= 0 ? P.insts[I.bsrc].oclass : operandClassOf(pi.B, bp);
     auto fill = [&](const PlanOperand &o, uint8_t &kind, uint8_t &col, uint8_t &valid, uint32_t &k) {
       kind = o.Kind; col = o.Column; valid = o.ConstValid;
       if (o.Kind == PLAN_OPERAND_COLUMN) P.cols[o.Column].used = 1;
@@ -979,13 +984,15 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P, Agg
       evalUnary(pi.Functor, z, (ValClass)acls, &rc);
       I.rclass = rc;
     }
+    // the first kJitMaxMagic fast divisions of the plan take a magic slot each; the others run the functor
+    I.magic = (int8_t)(isFastDiv(I) && nmagic < kJitMaxMagic ? nmagic++ : -1);
     switch (pi.Sink) {
       case PLAN_SINK_STACK: {
         ValClass oc = sinkClassOf(pi.SinkDataType, false);
         if (oc != VC_I32 && oc != VC_U32 && oc != VC_F32) throw EngineError("stack temporaries are Int32/Uint32/Float32");
         if ((int)stack.size() >= ARES_PLAN_STACK_DEPTH) throw EngineError("plan exceeds the evaluation stack depth");
         I.oclass = oc;
-        stack.push_back(oc);
+        stack.push_back(i);
         break;
       }
       case PLAN_SINK_FILTER:
@@ -1083,13 +1090,7 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P, Agg
   P.aggOp = st->op;
   {  // can a reached accumulator return to the neutral element?  (global dense slots carry no "reached" flags)
     bool safe = st->op != OP_SUM_I32 && st->op != OP_SUM_I64;   // float sums (-0.0), min / max (extreme), AVG (count 0)
-    if (!safe)   // integer sums: only of a positive literal (count(*)): never 0 again below 2^32 rows
-      for (int i = 0; i < P.ninsts; i++) {
-        const DevInst &I = P.insts[i];
-        if (I.sink == PLAN_SINK_MEASURE && !I.wide && I.nops == 1 && I.fn == Noop && I.akind == OPK_CONST && I.avalid &&
-            (I.aclass == VC_I32 || I.aclass == VC_U32) && (int32_t)I.aconst > 0)
-          safe = true;
-      }
+    for (int i = 0; i < P.ninsts; i++) safe = safe || positiveLiteralSum(P.insts[i], st->op);   // integer sums: count(*)
     P.neutralSafe = safe && !st->hll;
   }
   P.measWidth = (uint8_t)st->measWidth;
@@ -1211,7 +1212,7 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
   P.bypassOk = (P.hll || expectedGroups > 4 * slots) ? 1 : 0;
   // zone map known for every dimension: no key table, slots addressed by dimension value (jit.cu)
   P.denseGlobal = 0;
-  jitAnalyzeDense(P, P.bypassOk != 0);
+  jitAnalyzeDense(P);
   auto stageBytesFor = [&](uint32_t tr) {
     size_t stage = 0;
     for (int c = 0; c < P.ncols; c++) {
@@ -1682,25 +1683,14 @@ static void checkSharedStates(AggState *const *sts, int n, const BatchPlan &bp) 
 // The plan of the states in `set` (bit k = state k): every instruction except the other states' measure, member filter
 // and member dimension roots and the sub-expressions only they consume.  The kept states are renumbered in order; their
 // member dimensions become PLAN_SINK_DIMENSION roots (ordinals in plan order: the states of a set have the same
-// dimensions), and the member filters of a single state become ordinary filters.
-static void measurePlan(const BatchPlan &bp, uint32_t set, BatchPlan &out) {
-  std::vector<std::vector<int>> stack;   // instructions of each stacked sub-expression
-  std::vector<bool> drop(bp.NumInsts, false);
+// dimensions), and the member filters of a single state become ordinary filters.  `P` is `bp` compiled.
+static void measurePlan(const DevPlan &P, const BatchPlan &bp, uint32_t set, BatchPlan &out) {
+  bool drop[ARES_MAX_PLAN_INSTS] = {};
   for (int i = 0; i < bp.NumInsts; i++) {
     const PlanInst &pi = bp.Insts[i];
-    std::vector<int> tree{i};
-    auto pop = [&] {
-      if (stack.empty()) throw EngineError("plan pops an empty evaluation stack");
-      tree.insert(tree.end(), stack.back().begin(), stack.back().end());
-      stack.pop_back();
-    };
-    if (pi.NumOperands == 2 && pi.B.Kind == PLAN_OPERAND_STACK) pop();
-    if (pi.A.Kind == PLAN_OPERAND_STACK) pop();
-    if (pi.Sink == PLAN_SINK_STACK) stack.push_back(tree);
     const bool other = ((pi.Sink == PLAN_SINK_MEASURE || pi.Sink == PLAN_SINK_MEASURE_FILTER) && !((set >> pi.SinkArg) & 1u)) ||
                        (pi.Sink == PLAN_SINK_MEMBER_DIMENSION && (pi.SinkArg & set) == 0);
-    if (other)
-      for (int j : tree) drop[j] = true;
+    if (other) forSubexpression(P, i, [&](int j) { drop[j] = true; });
   }
   const bool single = (set & (set - 1)) == 0;
   auto rank = [&](int k) { return (uint8_t)__builtin_popcount(set & ((1u << k) - 1u)); };
@@ -1775,7 +1765,7 @@ static void scheduleStates(Schedule &S, AggState *const *sts, int n, const Batch
   uint32_t expected = 0;
   for (int k = 0; k < n; k++) {
     own[k] = &S.newPlan();
-    measurePlan(bp, 1u << k, *own[k]);
+    measurePlan(P, bp, 1u << k, *own[k]);
     Q[k] = &S.newDevPlan();
     compilePlan(sts[k], *own[k], *Q[k]);
     describeInputs(*Q[k], *own[k]);
@@ -1808,7 +1798,7 @@ static void scheduleStates(Schedule &S, AggState *const *sts, int n, const Batch
     for (int k = 0; k < n; k++)
       if ((mask >> k) & 1u) ss[m++] = sts[k];
     BatchPlan &plan = S.newPlan();
-    measurePlan(bp, mask, plan);
+    measurePlan(P, bp, mask, plan);
     DevPlan &Q1 = S.newDevPlan();
     compilePlan(ss[0], plan, Q1, ss, m);
     scheduleStates(S, ss, m, plan, Q1, true);
@@ -1830,7 +1820,7 @@ static const Schedule &scheduleBatch(AggState *const *sts, int n, const BatchPla
   const BatchPlan *plan = &bp;
   if (n == 1 && multi && (hasSink(bp, PLAN_SINK_MEASURE_FILTER) || hasSink(bp, PLAN_SINK_MEMBER_DIMENSION))) {
     BatchPlan &one = S.newPlan();
-    measurePlan(bp, 1u, one);
+    measurePlan(P, bp, 1u, one);
     compilePlan(sts[0], one, P);
     plan = &one;
   }

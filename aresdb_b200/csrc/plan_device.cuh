@@ -44,7 +44,9 @@ struct DevInst {
   uint8_t rclass;   // class of the functor result
   uint8_t oclass;   // class of the sink element
   uint8_t wide;     // 1: 8/16-byte column copied verbatim into a dimension
-  uint8_t rowOff, width, nullOff, pad;
+  uint8_t rowOff, width, nullOff;
+  int8_t magic;       // slot in JitParams::magic of a fast division (isFastDiv), -1: none
+  int8_t asrc, bsrc;  // instruction that pushed the value a stack operand pops, -1: not a stack operand
 };
 
 // One measure root of a plan: what the single-measure plan of its state decided (compilePlan + layoutStages on that plan),
@@ -117,6 +119,27 @@ struct DevPlan {
   DevMeasure meas[kJitMaxMeasures];
 };
 
+// Calls f(j) for instruction i and every instruction whose pushed value it consumes, directly or through others.
+template <class F>
+void forSubexpression(const DevPlan &P, int i, const F &f) {
+  f(i);
+  if (P.insts[i].asrc >= 0) forSubexpression(P, P.insts[i].asrc, f);
+  if (P.insts[i].bsrc >= 0) forSubexpression(P, P.insts[i].bsrc, f);
+}
+
+// Div / Mod / Floor of an integer class by a literal: strength-reduced with a magic multiplier (DevInst::magic)
+inline bool isFastDiv(const DevInst &I) {
+  return I.nops == 2 && (I.fn == Mod || I.fn == Floor || I.fn == Divide) && I.bkind == OPK_CONST &&
+         (I.tclass == VC_I32 || I.tclass == VC_U32) && (I.bclass == VC_I32 || I.bclass == VC_U32);
+}
+
+// count(*) and other sums of a positive literal: the sum never returns to 0 (below 2^32 rows), so a slot is reached iff
+// it is non-zero
+inline bool positiveLiteralSum(const DevInst &I, uint8_t aggOp) {
+  return I.sink == PLAN_SINK_MEASURE && !I.wide && (aggOp == OP_SUM_I32 || aggOp == OP_SUM_I64) && I.nops == 1 && I.fn == Noop &&
+         I.akind == OPK_CONST && I.avalid && (I.aclass == VC_I32 || I.aclass == VC_U32) && (int32_t)I.aconst > 0;
+}
+
 constexpr uint32_t kDenseMaxSlots = 8192;   // = slots of a CTA's accumulator slice in AggState::ctaAcc
 constexpr uint32_t kFxMaxRowsPerCta = 1u << 21;   // each 32-bit piece accumulator takes 2^21 adds of an 11-bit piece
 constexpr uint32_t kGlobalDenseMaxSlots = 1u << 21;   // 16 MB of accumulators per state, allocated on first use
@@ -124,7 +147,7 @@ constexpr uint32_t kGlobalDenseMaxSlots = 1u << 21;   // 16 MB of accumulators p
 // jit.cu: the fused kernel specialised for the plan's shape.  jitLaunch runs a batch on it and throws EngineError when
 // the kernel cannot be built (libnvrtc missing, the shape's compile failed: reported again for every batch of that
 // shape without compiling it twice); jitCompileOnly generates and compiles it without a GPU (AresJitDryRun).
-void jitAnalyzeDense(DevPlan &P, bool bypass);
+void jitAnalyzeDense(DevPlan &P);
 size_t jitCompileOnly(const DevPlan &P, std::string *sourceOut);
 void jitLaunch(const DevPlan &P, const DevTable &G, size_t smemBytes, int grid, cudaStream_t s);
 
