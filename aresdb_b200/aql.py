@@ -7,6 +7,8 @@ query's time range (UTC, numeric offsets like "-8" / "05:30", or an IANA name wi
                           expressions -> `col >= from AND col < to`)
 * time bucketizers        query/time_bucketizer.go:36-299, query/common/time_bucketizer.go:60-140
                           (regular -> FLOOR, recurring -> FLOOR(MOD) [/ unit], irregular -> calendar functors)
+* numeric bucketizers     query/common/aql.go:24-45 (bucketWidth / logBase / manualPartitions -> E.Bucket, a plan-only
+                          functor of the fused path; the dimension is the bucket ordinal, formatted as its lower bound)
 * measures                query/aql_compiler.go:1139-1250 (count -> sum(1), sum widening, hll) and
                           query/context/query_context_helper.go:540-575 (countdistincthll)
 * row / common filters    SQL-ish boolean expressions over columns and literals with the reference parser's operator
@@ -36,6 +38,7 @@ from __future__ import annotations
 
 import calendar
 import datetime as _dt
+import math
 import re
 from dataclasses import dataclass, field
 
@@ -647,6 +650,10 @@ def compile_query(query: dict, table: Table, now: int, reduce_mode: int = A.ARES
     dims = []
     for d in query.get("dimensions") or []:
         e = parse_expression(d.get("sqlExpression") or d.get("expr"), table, foreign)
+        if d.get("numericBucketizer"):
+            if d.get("timeBucketizer"):
+                raise AQLError("a dimension has a timeBucketizer or a numericBucketizer, not both")
+            e = numeric_bucket_expr(d["numericBucketizer"], e, table, upload)
         if d.get("timeBucketizer"):
             if tz_operand is not None:      # (timeColumn CONVERT_TZ timezoneColumn): the joined row's offset
                 e = E.Binary(A.Plus, e, tz_operand)
@@ -680,6 +687,102 @@ def time_bucket_start(ts: int, bucketizer: str) -> int:
     if bucketizer == "week":   # Monday 00:00 (reference query/functor.cu:207-212)
         return ts - (ts - SECONDS_PER_4_DAYS) % SECONDS_PER_WEEK
     return ts - ts % _regular_bucket_seconds(bucketizer)
+
+
+# ---- numeric bucketizer ------------------------------------------------------------------------------
+FLT_MAX = 3.4028234663852886e38
+MAX_LOG_BOUNDS = 65536        # a log table's ordinals are Uint16
+MAX_PARTITIONS = 255          # manual partitions' ordinals are Uint8
+
+
+def _number(v, what: str) -> float:
+    if isinstance(v, bool) or not isinstance(v, (int, float)):
+        raise AQLError(f"numericBucketizer: {what} must be a number")
+    return float(v)
+
+
+def _pow(b: float, k: int) -> float:
+    try:
+        return b ** k
+    except OverflowError:
+        return math.inf
+
+
+def log_table(b: float, is_float: bool) -> tuple:
+    """(exponent of t[0], t): the bounds t[j] = b ** (kmin + j) of a log-base bucketizer, strictly increasing, covering the
+    positive values of the operand's class: from t[0] <= 2^-149 to t[-1] > FLT_MAX for Float32 values, from t[0] <= 1 to
+    t[-1] > 2^32 for integers."""
+    lo, hi = (2.0 ** -149, FLT_MAX) if is_float else (1.0, 2.0 ** 32)
+    k = math.floor(math.log(lo) / math.log(b))
+    while _pow(b, k) > lo:
+        k -= 1
+    while _pow(b, k + 1) <= lo:
+        k += 1
+    t = [_pow(b, k)]
+    while t[-1] <= hi:
+        if len(t) >= MAX_LOG_BOUNDS:
+            raise AQLError(f"numericBucketizer: logBase {b!r} needs more than {MAX_LOG_BOUNDS} buckets")
+        t.append(_pow(b, k + len(t)))
+    if any(x >= y for x, y in zip(t, t[1:])):
+        raise AQLError(f"numericBucketizer: the bounds of logBase {b!r} are not strictly increasing")
+    return k, tuple(t)
+
+
+def numeric_bucket_expr(defn, e: E.Expr, table: Table, upload=None) -> E.Expr:
+    """numericBucketizer (NumericBucketizerDef, query/common/aql.go:24-45) of dimension expression `e` -> E.Bucket.  As in
+    the Go struct, a zero field is an unset field, and nothing set ({}) leaves the dimension as it is.  The bounds of the
+    log-base and manual-partition forms go to the executor's memory space through `upload(float64 array) -> buffer with
+    .ptr`."""
+    if not isinstance(defn, dict):
+        raise AQLError("numericBucketizer must be an object")
+    unknown = set(defn) - {"bucketWidth", "logBase", "manualPartitions"}
+    if unknown:
+        raise AQLError(f"numericBucketizer: unknown field {sorted(unknown)[0]}")
+    width, base, parts = defn.get("bucketWidth") or 0, defn.get("logBase") or 0, defn.get("manualPartitions") or []
+    given = [name for name, v in (("bucketWidth", width), ("logBase", base), ("manualPartitions", parts)) if v]
+    if not given:
+        return e
+    if len(given) > 1:
+        raise AQLError("numericBucketizer: set one of bucketWidth, logBase and manualPartitions")
+    r = E.resolve(e)
+    if E.uses_foreign(r):
+        raise AQLError("numericBucketizer: a joined table's column cannot be bucketized")
+    if isinstance(r, E.Col) and (table.columns[r.index].enum is not None or table.columns[r.index].hll):
+        raise AQLError(f"numericBucketizer: {table.columns[r.index].name} is an enum or hll column")
+    if r.type not in (E.Type.Boolean, E.Type.Unsigned, E.Type.Signed, E.Type.Float) or E.dimension_data_type(r) in (A.Int64, A.UUID):
+        raise AQLError("numericBucketizer: the dimension must be a Bool, 1-, 2-, 4-byte integer or Float32 value")
+    if width:
+        w = _number(width, "bucketWidth")
+        if not (0 < w < math.inf):
+            raise AQLError("numericBucketizer: bucketWidth must be finite and > 0")
+        return E.Bucket(e, ("width", w))
+    if base:
+        b = _number(base, "logBase")
+        if not (1 < b < math.inf):
+            raise AQLError("numericBucketizer: logBase must be finite and > 1")
+        kmin, bounds = log_table(b, r.type == E.Type.Float)
+        spec = ("log", b, kmin, len(bounds))
+    else:
+        if not isinstance(parts, list) or not 1 <= len(parts) <= MAX_PARTITIONS:
+            raise AQLError(f"numericBucketizer: manualPartitions must be a list of 1 to {MAX_PARTITIONS} numbers")
+        bounds = tuple(_number(p, "a manual partition") for p in parts)
+        if not all(-math.inf < p < math.inf for p in bounds) or any(x >= y for x, y in zip(bounds, bounds[1:])):
+            raise AQLError("numericBucketizer: manualPartitions must be finite and strictly increasing")
+        spec = ("partitions",) + bounds
+    if upload is None:
+        raise AQLError("numericBucketizer: the bounds need `upload` (they live in the executor's memory space)")
+    import numpy as np
+    buf = upload(np.array(bounds, np.float64))
+    return E.Bucket(e, spec, bounds, buf.ptr, buf)
+
+
+def bucket_lower_bound(spec: tuple, ordinal: int) -> float:
+    """The lower bound of bucket `ordinal` of a numeric bucketizer (E.Bucket.spec): fl(k * w), t[j], or -inf / p[i - 1]."""
+    if spec[0] == "width":
+        return float(ordinal) * spec[1]
+    if spec[0] == "log":
+        return _pow(spec[1], spec[2] + ordinal)
+    return -math.inf if ordinal == 0 else spec[ordinal]
 
 
 def compile_request(request, table: Table, now: int, **kwargs) -> list:

@@ -169,7 +169,7 @@ class PlanOperand(C.Structure):
 
 class PlanInst(C.Structure):
     _fields_ = [("NumOperands", C.c_uint8), ("Functor", C.c_uint8), ("Sink", C.c_uint8),
-                ("SinkArg", C.c_uint8), ("SinkDataType", C.c_uint8), ("Reserved", C.c_uint8 * 3),
+                ("SinkArg", C.c_uint8), ("SinkDataType", C.c_uint8), ("Bucket", C.c_uint8), ("Reserved", C.c_uint8 * 2),
                 ("A", PlanOperand), ("B", PlanOperand)]
 
 
@@ -179,6 +179,16 @@ class ColumnRange(C.Structure):
 
 
 ARES_MAX_FOREIGN_TABLES, ARES_MAX_FOREIGN_COLUMNS = 4, 8
+
+# plan-only unary functor: the numeric bucketizer BatchPlan.Bucketizers[PlanInst.Bucket] (batch_plan.h)
+PLAN_FN_NUMERIC_BUCKET = 200
+PLAN_BUCKET_WIDTH, PLAN_BUCKET_LOG, PLAN_BUCKET_PARTITIONS = 1, 2, 3
+ARES_MAX_PLAN_BUCKETIZERS = 4
+
+
+class PlanBucketizer(C.Structure):
+    _fields_ = [("Kind", C.c_uint8), ("Reserved", C.c_uint8 * 3), ("LogMin", C.c_int32), ("Param", C.c_double),
+                ("Bounds", C.c_void_p), ("NumBounds", C.c_uint32), ("Reserved2", C.c_uint32)]
 
 
 class PlanForeignTable(C.Structure):
@@ -195,7 +205,8 @@ class BatchPlan(C.Structure):
                 ("BaseCounts", C.c_void_p), ("StartCount", C.c_uint32), ("NumRows", C.c_uint32),
                 ("Ranges", ColumnRange * ARES_MAX_PLAN_COLUMNS),
                 ("ForeignTables", PlanForeignTable * ARES_MAX_FOREIGN_TABLES), ("NumForeignTables", C.c_int32),
-                ("ForeignColumns", PlanForeignColumn * ARES_MAX_FOREIGN_COLUMNS), ("NumForeignColumns", C.c_int32)]
+                ("ForeignColumns", PlanForeignColumn * ARES_MAX_FOREIGN_COLUMNS), ("NumForeignColumns", C.c_int32),
+                ("Bucketizers", PlanBucketizer * ARES_MAX_PLAN_BUCKETIZERS), ("NumBucketizers", C.c_int32)]
 
 
 class AggSpec(C.Structure):

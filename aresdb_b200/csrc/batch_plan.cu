@@ -918,6 +918,37 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P, Agg
     if (t < 0 || t >= bp.NumForeignTables) throw EngineError("foreign column of a table outside BatchPlan.ForeignTables");
     P.foreignTableOf[k] = (uint8_t)t;
   }
+  // numeric bucketizers: the parameters are checked here, the bounds tables (device memory) are the caller's
+  if (bp.NumBucketizers < 0 || bp.NumBucketizers > kJitMaxBuckets) throw EngineError("invalid number of numeric bucketizers");
+  P.nbuckets = (uint8_t)bp.NumBucketizers;
+  for (int j = 0; j < bp.NumBucketizers; j++) {
+    const PlanBucketizer &B = bp.Bucketizers[j];
+    const double v = B.Param;
+    switch (B.Kind) {
+      case PLAN_BUCKET_WIDTH:
+        if (!(v > 0.0 && v <= kMaxFinite)) throw EngineError("numeric bucketizer " + std::to_string(j) + ": the width must be finite and > 0");
+        break;
+      case PLAN_BUCKET_LOG:
+        if (!(v > 1.0 && v <= kMaxFinite)) throw EngineError("numeric bucketizer " + std::to_string(j) + ": the log base must be finite and > 1");
+        if (!B.Bounds || B.NumBounds < 2 || B.NumBounds > 65537)
+          throw EngineError("numeric bucketizer " + std::to_string(j) + ": a log table has 2..65537 bounds in device memory");
+        break;
+      case PLAN_BUCKET_PARTITIONS:
+        if (!B.Bounds || B.NumBounds < 1 || B.NumBounds > 255)
+          throw EngineError("numeric bucketizer " + std::to_string(j) + ": manual partitions are 1..255 bounds in device memory");
+        break;
+      default: throw EngineError("numeric bucketizer " + std::to_string(j) + ": unknown kind");
+    }
+    P.bucketKind[j] = B.Kind;
+    P.bucketSlot[j] = 0xFF;
+    JitBucket &D = P.buckets[j];
+    D.bounds = B.Bounds;
+    D.param = v;
+    D.n = B.NumBounds;
+    D.logMin = B.LogMin;
+    D.invLog2 = B.Kind == PLAN_BUCKET_LOG ? (float)(1.0 / log2(v)) : 0.0f;
+  }
+  int nbucketSlots = 0;
   const DimLayout &RL = st->rowLayout;
   std::vector<int> stack;   // the instructions whose pushed values are on the evaluation stack
   std::vector<bool> dimSeen(RL.numDims, false);
@@ -977,6 +1008,21 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P, Agg
       ValClass rc;
       evalBinary(pi.Functor, z, z, (ValClass)I.tclass, &rc);
       I.rclass = rc;
+    } else if (pi.Functor == PLAN_FN_NUMERIC_BUCKET) {
+      // a dimension root over a 32-bit (or Bool) value whose sink type is the ordinal type of the bucketizer's kind
+      if (pi.NumOperands != 1) throw EngineError("PLAN_FN_NUMERIC_BUCKET is a unary functor");
+      if (pi.Bucket >= bp.NumBucketizers) throw EngineError("PLAN_FN_NUMERIC_BUCKET names a bucketizer outside BatchPlan.Bucketizers");
+      if (pi.Sink != PLAN_SINK_DIMENSION && pi.Sink != PLAN_SINK_MEMBER_DIMENSION) throw EngineError("a numeric bucketizer is a dimension root");
+      if (acls != VC_BOOL && acls != VC_I32 && acls != VC_U32 && acls != VC_F32)
+        throw EngineError("a numeric bucketizer's operand is a Bool, 1-, 2-, 4-byte integer or Float32 value");
+      const uint8_t kind = P.bucketKind[pi.Bucket];
+      const int dt = kind == PLAN_BUCKET_WIDTH ? Int32 : kind == PLAN_BUCKET_LOG ? Uint16 : Uint8;
+      if (pi.SinkDataType != dt)
+        throw EngineError("a numeric bucketizer's dimension is Int32 (width), Uint16 (log base) or Uint8 (manual partitions)");
+      if (kind == PLAN_BUCKET_PARTITIONS && P.bucketSlot[pi.Bucket] == 0xFF) P.bucketSlot[pi.Bucket] = (uint8_t)nbucketSlots++;
+      I.bucket = pi.Bucket;
+      I.tclass = acls;
+      I.rclass = sinkClassOf(dt, true);
     } else {
       I.tclass = acls;
       Cell z; z.v = 0; z.valid = true;
@@ -1074,6 +1120,7 @@ static void compilePlan(const AggState *st, const BatchPlan &bp, DevPlan &P, Agg
     }
   }
   if (!stack.empty()) throw EngineError("plan leaves values on the evaluation stack");
+  P.bucketSmem = (uint32_t)nbucketSlots * kBucketSmemBytes;
   for (int d = 0; d < RL.numDims && !P.memberDims; d++)
     if (!dimSeen[d]) throw EngineError("plan does not produce every dimension of AggSpec");
   for (int k = 0; k < nmulti && P.memberDims; k++)
@@ -1203,6 +1250,8 @@ static bool memberSlots(DevPlan &P, size_t avail) {
 // A single-measure plan describes its measure in meas[0].
 static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
   const bool stageBc = stagesBaseCounts(P);
+  // (partition tables of numeric bucketizers sit after the stages)
+  const size_t budget = (size_t)kSmemBudget - P.bucketSmem;
   // The shared table takes 8192 slots (128 KB) whenever a ring of >= 2 stages still fits beside
   // it: measured on cfg3 (2,400 groups per batch) 8192 slots beat 4096 by 1.5x because fewer
   // probe iterations are paid per warp; a plan with very wide rows falls back to fewer slots.
@@ -1240,9 +1289,9 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
       for (uint32_t n = kMaxStages; n >= 2 && !tileRows; n--) {
         // (several measures: one 128-byte aligned region of accumulators each)
         const size_t need = 128 + n * stageBytesFor(tr) + (P.nmeas > 1 && !P.memberDims ? 128 * P.nmeas : 0);
-        if (need >= (size_t)kSmemBudget) continue;
+        if (need >= budget) continue;
         if (P.memberDims) {   // (only with several measures: scheduleStates)
-          if (memberSlots(P, (size_t)kSmemBudget - need)) {
+          if (memberSlots(P, budget - need)) {
             tileRows = tr; stages = n; slots = 16;
             for (int m = 0; m < P.nmeas; m++) slots = P.meas[m].slots > slots ? P.meas[m].slots : slots;
           }
@@ -1254,7 +1303,7 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
           slotBytes = 0;
           for (int m = 0; m < P.nmeas; m++) slotBytes += P.meas[m].denseFx ? 12 : 9;
         }
-        uint32_t cap = (uint32_t)(((size_t)kSmemBudget - need) / slotBytes / 16 * 16);
+        uint32_t cap = (uint32_t)((budget - need) / slotBytes / 16 * 16);
         if (cap > kDenseMaxSlots) cap = kDenseMaxSlots;
         if (cap >= P.denseTotal) { tileRows = tr; stages = n; slots = cap; }
       }
@@ -1263,7 +1312,7 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
     if (!tileRows && !P.hll && P.nmeas <= 1 && P.neutralSafe && P.denseTotal <= kGlobalDenseMaxSlots) {
       // more slots than a CTA holds: one accumulator array in global memory for the whole grid; shared memory is all ring
       for (uint32_t tr : {3968u, 1920u, 896u}) {
-        const uint32_t n = stagesIn((size_t)kSmemBudget - 128 - 256, tr);
+        const uint32_t n = stagesIn(budget - 128 - 256, tr);
         if (n >= 2) {
           tileRows = tr; stages = n; slots = 16; P.denseGlobal = 1; P.denseFx = 0;
           // L2 atomics saturate at >= ~1M distinct addresses and contend below (tools/microbench/agg_microbench.cu):
@@ -1283,7 +1332,7 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
   if (!tileRows) {
     for (uint32_t sl : {slots, slots / 2, slots / 4}) {
       for (uint32_t tr : {3968u, 1920u, 896u}) {  // 128 rows x (31 | 15 | 7) consumer warps
-        const uint32_t n = stagesIn((size_t)kSmemBudget - 128 - (size_t)sl * 8, tr);
+        const uint32_t n = stagesIn(budget - 128 - (size_t)sl * 8, tr);
         if (n >= 2) { tileRows = tr; stages = n; break; }
       }
       if (tileRows) { slots = sl; break; }
@@ -1328,7 +1377,7 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
   } else {
     describeMeasure(P, P.meas[0]);
   }
-  return 128 + (size_t)P.tableBytes + stageBytes * P.numStages;
+  return 128 + (size_t)P.tableBytes + stageBytes * P.numStages + P.bucketSmem;
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1616,7 +1665,7 @@ static void executePlan(const Launch &L, cudaStream_t s) {
       P.meas[k].ctaAcc = L.sts[k]->ctaAcc;
     }
     P.ctaAcc = st->ctaAcc;
-    jitLaunch(P, st->table, 128 + (size_t)P.tableBytes + (size_t)P.stageBytes * P.numStages, launchGrid(P), s);
+    jitLaunch(P, st->table, 128 + (size_t)P.tableBytes + (size_t)P.stageBytes * P.numStages + P.bucketSmem, launchGrid(P), s);
     if (P.denseGlobal) {
       DenseFold F;
       memset(&F, 0, sizeof(F));

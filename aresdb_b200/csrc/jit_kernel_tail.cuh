@@ -536,6 +536,9 @@ extern "C" __global__ void __launch_bounds__(JIT_THREADS, 1) aresFusedJit(const 
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
+#ifdef JIT_BUCKETS
+  jitStageBuckets(P);   // partition tables of the plan's numeric bucketizers
+#endif
   __syncthreads();
 
   // Warp specialisation: the last warp is the TMA producer (one lane issues the bulk copies as soon

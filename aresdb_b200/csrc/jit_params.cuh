@@ -4,6 +4,7 @@
 #pragma once
 #include "fused_device.cuh"
 #include "join.cuh"
+#include "numeric_bucket.cuh"
 
 namespace aresb {
 
@@ -74,6 +75,7 @@ struct JitParams {
   // dimension m does not have); lane-private copies of its slots, mRepStride[m] slots apart
   uint32_t mStride[kJitMaxMeasures][kJitMaxDenseDims];
   uint32_t mReps[kJitMaxMeasures], mRepStride[kJitMaxMeasures];
+  JitBucket bk[kJitMaxBuckets];           // the plan's numeric bucketizers (BatchPlan.Bucketizers)
 };
 // (with every measure's group table in it: the block stays far below the 32 KB kernel-parameter limit of sm_90)
 static_assert(sizeof(JitParams) <= 4096, "the kernel's parameter block is limited to 4 KB");

@@ -47,6 +47,7 @@ struct DevInst {
   uint8_t rowOff, width, nullOff;
   int8_t magic;       // slot in JitParams::magic of a fast division (isFastDiv), -1: none
   int8_t asrc, bsrc;  // instruction that pushed the value a stack operand pops, -1: not a stack operand
+  uint8_t bucket;     // PLAN_FN_NUMERIC_BUCKET: index into DevPlan::buckets
 };
 
 // One measure root of a plan: what the single-measure plan of its state decided (compilePlan + layoutStages on that plan),
@@ -117,6 +118,12 @@ struct DevPlan {
   uint8_t nmeas;           // > 1: measure roots feeding that many states (direct-indexed form only); meas[] describes them
   uint8_t memberDims;      // PLAN_SINK_MEMBER_DIMENSION roots of the plan (0: plain dimension roots; the states differ in theirs)
   DevMeasure meas[kJitMaxMeasures];
+  // numeric bucketizers (BatchPlan.Bucketizers): kind, the kernel's descriptor, and for partition tables their
+  // kBucketSmemBytes slot in the shared memory after the stages (bucketSmem bytes in all, staged once per CTA)
+  uint8_t nbuckets;
+  uint8_t bucketKind[kJitMaxBuckets], bucketSlot[kJitMaxBuckets];
+  uint32_t bucketSmem;
+  JitBucket buckets[kJitMaxBuckets];
 };
 
 // Calls f(j) for instruction i and every instruction whose pushed value it consumes, directly or through others.

@@ -74,6 +74,8 @@ class LegacyBatchExecutor:
     """The reference's one-operator-per-kernel call sequence, batch after batch."""
 
     def __init__(self, lib: A.Library, space, query: AggQuery):
+        if any(E.uses_bucket(d) for d in query.dimensions):
+            raise ValueError("numeric bucketizers run on the fused path only: the per-node call sequence has no such functor")
         self.lib, self.space, self.q = lib, space, query
         self.result_size = 0
         self.out: _ResultBuffers | None = None   # results of the batches processed so far
@@ -340,6 +342,19 @@ class _BatchPlans:
         for i, pi in enumerate(self.insts):
             self._plan.Insts[i] = pi
         self._plan_variants = {}
+        # numeric bucketizers: parameters, and their bounds in the executor's memory space (uploaded by the front-end)
+        self._plan.NumBucketizers = len(query.bucketizers)
+        for j, b in enumerate(query.bucketizers):
+            pb = self._plan.Bucketizers[j]
+            pb.Kind = {"width": A.PLAN_BUCKET_WIDTH, "log": A.PLAN_BUCKET_LOG, "partitions": A.PLAN_BUCKET_PARTITIONS}[b.kind]
+            if b.kind != "partitions":
+                pb.Param = b.spec[1]
+            if b.kind == "log":
+                pb.LogMin = b.spec[2]
+            if b.kind != "width":
+                if not b.bounds_ptr:
+                    raise ValueError("a numeric bucketizer's bounds are not in the executor's memory space (bounds_ptr)")
+                pb.Bounds, pb.NumBounds = b.bounds_ptr, len(b.bounds)
         # joined dimension tables: the lookup + foreign-column reads are a gather stage of the fused kernel
         self._join_keep = []
         if query.joins:

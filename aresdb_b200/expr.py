@@ -84,6 +84,32 @@ class Binary(Expr):
     type: Type = Type.Unknown
 
 
+@dataclass
+class Bucket(Expr):
+    """A numeric bucketizer over `expr` (PLAN_FN_NUMERIC_BUCKET, a dimension root): the dimension holds the bucket ordinal.
+    `spec` is the bucketizer's identity: ("width", w), ("log", b, log_min, number of bounds) or ("partitions", p0, ...).
+    `bounds` is the log table / the partitions as doubles, `bounds_ptr` their copy in the executor's memory space (what
+    BatchPlan.Bucketizers points at); neither is part of the expression's identity beyond `spec`."""
+    expr: Expr
+    spec: tuple
+    bounds: tuple = field(default=(), repr=False, compare=False)
+    bounds_ptr: int = field(default=0, repr=False, compare=False)
+    keep: object = field(default=None, repr=False, compare=False)   # the device copy of the bounds
+
+    @property
+    def kind(self) -> str:
+        return self.spec[0]
+
+    @property
+    def type(self):
+        return Type.Signed if self.kind == "width" else Type.Unsigned
+
+    @property
+    def data_type(self) -> int:
+        """Type of the ordinal: Int32 (width), Uint16 (log base), Uint8 (manual partitions)."""
+        return {"width": A.Int32, "log": A.Uint16, "partitions": A.Uint8}[self.kind]
+
+
 def _cast(e: Expr, t: Type) -> Expr:
     """expr.Cast: literals change type in place; other nodes keep theirs (the functor promotes)."""
     if isinstance(e, Lit) and t in (Type.Float, Type.Signed, Type.Unsigned) and e.type != t:
@@ -99,6 +125,8 @@ def resolve(e: Expr) -> Expr:
     """Bottom-up type resolution (returns a new tree)."""
     if isinstance(e, (Col, Lit, ForeignCol)):
         return e
+    if isinstance(e, Bucket):
+        return Bucket(resolve(e.expr), e.spec, e.bounds, e.bounds_ptr, e.keep)
     if isinstance(e, Unary):
         c = resolve(e.expr)
         t = c.type
@@ -149,7 +177,7 @@ def scratch_data_type(t: Type) -> int:
 
 def dimension_data_type(e: Expr) -> int:
     """GetDimensionDataType — reference query/common/dim_util.go:9-40."""
-    if isinstance(e, (Col, ForeignCol)):
+    if isinstance(e, (Col, ForeignCol, Bucket)):
         return e.data_type
     return {Type.Boolean: A.Bool, Type.Unsigned: A.Uint32, Type.Signed: A.Int32, Type.Float: A.Float32,
             Type.UUID: A.UUID}.get(e.type, A.Uint32)
@@ -175,8 +203,19 @@ def uses_foreign(e: Expr) -> bool:
     """Does the expression read a joined table's column?"""
     if isinstance(e, ForeignCol):
         return True
-    if isinstance(e, Unary):
+    if isinstance(e, (Unary, Bucket)):
         return uses_foreign(e.expr)
     if isinstance(e, Binary):
         return uses_foreign(e.lhs) or uses_foreign(e.rhs)
+    return False
+
+
+def uses_bucket(e: Expr) -> bool:
+    """Is the expression a numeric bucketizer (or does it contain one)?"""
+    if isinstance(e, Bucket):
+        return True
+    if isinstance(e, Unary):
+        return uses_bucket(e.expr)
+    if isinstance(e, Binary):
+        return uses_bucket(e.lhs) or uses_bucket(e.rhs)
     return False

@@ -13,7 +13,8 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import cabi as A
-from .aql import _regular_bucket_seconds, AQLError, SECONDS_PER_4_DAYS
+from . import expr as E
+from .aql import _regular_bucket_seconds, AQLError, SECONDS_PER_4_DAYS, bucket_lower_bound
 from .query import HLL_REGISTERS, HLLResult, QueryResult
 
 NULL_STRING = "NULL"
@@ -28,6 +29,24 @@ class DimensionMeta:
     from_offset: int = 0                   # seconds the query's time zone is ahead of UTC (AggQuery.tz_offset)
     to_offset: int = 0                     # ... at the end of the range, and the switch instant when they differ
     dst_switch: int = 0                    # (AggQuery.tz_to_offset / dst_switch)
+    numeric_bucketizer: tuple | None = None  # E.Bucket.spec of a numeric bucketizer: the value is the bucket ordinal
+
+
+def format_float64(x) -> str:
+    """strconv.FormatFloat(v, 'g', -1, 64): the 64-bit sibling of format_float32 (shortest digits that round-trip a
+    double; exponent form when the decimal exponent is < -4 or >= 6)."""
+    f = float(x)
+    if math.isnan(f):
+        return "NaN"
+    if math.isinf(f):
+        return "+Inf" if f > 0 else "-Inf"
+    if f == 0:
+        return "-0" if math.copysign(1.0, f) < 0 else "0"
+    mant, exp = np.format_float_scientific(np.float64(f), unique=True, trim="-", exp_digits=2).split("e")
+    e = int(exp)
+    if e < -4 or e >= 6:
+        return f"{mant}e{'+' if e >= 0 else '-'}{abs(e):02d}"
+    return np.format_float_positional(np.float64(f), unique=True, trim="-")
 
 
 def format_float32(x) -> str:
@@ -89,6 +108,8 @@ def read_dimension(raw, valid, data_type: int, meta: DimensionMeta | None) -> st
     """One dimension value of one result row -> its string form (None for NULL)."""
     if not valid:
         return None
+    if meta is not None and meta.numeric_bucketizer is not None:
+        return format_float64(bucket_lower_bound(meta.numeric_bucketizer, int(raw)))
     is_time = meta is not None and meta.time_bucketizer is not None
     if data_type == A.Float32:
         if not is_time:
@@ -111,10 +132,15 @@ def read_dimension(raw, valid, data_type: int, meta: DimensionMeta | None) -> st
     return str(val)
 
 
+def default_metas(q) -> list:
+    """The formatting a query's dimensions carry by themselves: the lower bounds of numeric bucketizers."""
+    return [DimensionMeta(numeric_bucketizer=d.spec) if isinstance(d, E.Bucket) else None for d in q.dimensions]
+
+
 def nested_result(result: QueryResult, metas: list | None = None) -> dict:
     """QueryResult -> nested dict keyed by the formatted dimension values, leaves = float measures."""
     q = result.query
-    metas = metas or [None] * len(q.dimensions)
+    metas = metas or default_metas(q)
     cols = result.decoded_dims()
     out: dict = {}
     for g in range(result.groups):
@@ -181,7 +207,7 @@ def hll_estimate(dense: np.ndarray) -> float:
 
 def hll_nested_result(result: HLLResult, metas: list | None = None) -> dict:
     q = result.query
-    metas = metas or [None] * len(q.dimensions)
+    metas = metas or default_metas(q)
     cols = result.dims.decoded_dims()
     dense = result.dense_registers()
     out: dict = {}

@@ -138,6 +138,7 @@ class AggQuery:
         members = [self] if measures is None else measures
         insts: list[A.PlanInst] = []
         self.foreign_columns = []   # distinct (table, column, timezone) leaves in first-use order = BatchPlan.ForeignColumns
+        self.bucketizers = []       # distinct numeric bucketizers in first-use order = BatchPlan.Bucketizers
 
         def operand(e: E.Expr) -> A.PlanOperand:
             o = A.PlanOperand()
@@ -161,7 +162,16 @@ class AggQuery:
 
         def emit(e: E.Expr, sink: int, sink_arg: int, sink_dt: int):
             pi = A.PlanInst()
-            if isinstance(e, E.Binary):
+            if isinstance(e, E.Bucket):
+                if sink not in (A.PLAN_SINK_DIMENSION, A.PLAN_SINK_MEMBER_DIMENSION):
+                    raise ValueError("a numeric bucketizer is a dimension")
+                if e not in self.bucketizers:
+                    self.bucketizers.append(e)
+                if len(self.bucketizers) > A.ARES_MAX_PLAN_BUCKETIZERS:
+                    raise ValueError(f"at most {A.ARES_MAX_PLAN_BUCKETIZERS} numeric bucketizers per plan")
+                pi.NumOperands, pi.Functor, pi.A = 1, A.PLAN_FN_NUMERIC_BUCKET, operand(e.expr)
+                pi.Bucket = self.bucketizers.index(e)
+            elif isinstance(e, E.Binary):
                 a = operand(e.lhs)
                 b = operand(e.rhs)
                 pi.NumOperands, pi.Functor, pi.A, pi.B = 2, e.op, a, b
@@ -214,7 +224,8 @@ class AggQuery:
             dims = repr([(self.dimensions[qi], self.dim_types[qi]) for qi in self.dim_order])
             return dims, repr(self.filters[lo:hi]), joins, self.reduce_mode
         prefix = tuple(bytes(pi) for pi in self.plan_instructions(measures=[]))
-        return prefix, self.time_filter_range, joins, self.reduce_mode
+        # (an instruction names its bucketizer by index: the specs themselves tell two widths apart)
+        return prefix, repr([b.spec for b in self.bucketizers]), self.time_filter_range, joins, self.reduce_mode
 
 
 def member_dimensions(queries: list):

@@ -66,14 +66,42 @@ enum PlanSink {
                                   * member dimension roots with bit k (a member dimension, see ExecuteBatchPlanMulti) */
 };
 
+/* Plan-only unary functor (no UnaryFunctorType has this value): the numeric bucketizer BatchPlan.Bucketizers[Bucket]
+ * applied to the operand.  The instruction is a dimension root (PLAN_SINK_DIMENSION or PLAN_SINK_MEMBER_DIMENSION) whose
+ * SinkDataType is the ordinal type of the bucketizer's kind; its operand is a Bool, 1-, 2-, 4-byte integer or Float32
+ * value, compared as an exact double.  A NULL or NaN operand gives a NULL dimension. */
+enum { PLAN_FN_NUMERIC_BUCKET = 200 };
+
+enum PlanBucketizerKind {
+  PLAN_BUCKET_WIDTH = 1,      /* Param = w (finite, > 0): Int32 ordinal k with fl(k*w) <= x < fl((k+1)*w); +-inf and
+                               * ordinals outside Int32: NULL */
+  PLAN_BUCKET_LOG = 2,        /* Param = b (finite, > 1), Bounds = t[0..NumBounds-1] strictly increasing (t[j] = b^(LogMin+j)):
+                               * Uint16 ordinal j with t[j] <= x < t[j+1]; x <= 0, +inf and x outside the table: NULL */
+  PLAN_BUCKET_PARTITIONS = 3  /* Bounds = p[0..NumBounds-1] (1..255, finite, strictly increasing): Uint8 ordinal = the
+                               * number of p[i] <= x (-inf: 0, +inf: NumBounds) */
+};
+
 typedef struct {
-  uint8_t NumOperands;  /* 1: Functor is a UnaryFunctorType; 2: a BinaryFunctorType */
+  uint8_t Kind;          /* enum PlanBucketizerKind */
+  uint8_t Reserved[3];
+  int32_t LogMin;        /* PLAN_BUCKET_LOG: exponent of t[0] */
+  double Param;          /* w or b */
+  const double *Bounds;  /* device memory, valid until the batch's kernel has run (PLAN_BUCKET_LOG / PARTITIONS) */
+  uint32_t NumBounds;    /* PLAN_BUCKET_LOG: 2..65537; PLAN_BUCKET_PARTITIONS: 1..255 */
+  uint32_t Reserved2;
+} PlanBucketizer;
+
+enum { ARES_MAX_PLAN_BUCKETIZERS = 4 };
+
+typedef struct {
+  uint8_t NumOperands;  /* 1: Functor is a UnaryFunctorType (or PLAN_FN_NUMERIC_BUCKET); 2: a BinaryFunctorType */
   uint8_t Functor;
   uint8_t Sink;         /* enum PlanSink */
   uint8_t SinkArg;      /* dimension ordinal for PLAN_SINK_DIMENSION; state ordinal for PLAN_SINK_MEASURE and
                          * PLAN_SINK_MEASURE_FILTER (Multi); mask of states for PLAN_SINK_MEMBER_DIMENSION (Multi) */
   uint8_t SinkDataType; /* enum DataType of the sink element */
-  uint8_t Reserved[3];
+  uint8_t Bucket;       /* PLAN_FN_NUMERIC_BUCKET: index into BatchPlan.Bucketizers (0 otherwise) */
+  uint8_t Reserved[2];
   PlanOperand A;
   PlanOperand B;
 } PlanInst;
@@ -130,6 +158,8 @@ typedef struct {
   int32_t NumForeignTables;
   PlanForeignColumn ForeignColumns[ARES_MAX_FOREIGN_COLUMNS];
   int32_t NumForeignColumns;
+  PlanBucketizer Bucketizers[ARES_MAX_PLAN_BUCKETIZERS]; /* numeric bucketizers of PLAN_FN_NUMERIC_BUCKET instructions */
+  int32_t NumBucketizers;
 } BatchPlan;
 
 enum AresReduceMode {
