@@ -361,6 +361,7 @@ _PLAN_SIGS = {
     "AggStateExport": [_VP, DimensionVector, _VP, _VP, C.c_int],
     "AggStateFinalizeHLL": [_VP, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.POINTER(C.c_void_p),
                             _VP, C.c_int],
+    "AggStateFinalizeHLLEstimate": [_VP, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), _VP, C.c_int],
     "AggStateReset": [_VP, _VP, C.c_int],
     "AggStateDestroy": [_VP, C.c_int],
     "AggStatesFinalize": [C.POINTER(C.c_void_p), C.c_int, C.POINTER(DimensionVector), C.POINTER(C.c_void_p), C.POINTER(C.c_int64), _VP,

@@ -46,6 +46,8 @@ int hllRegisterVectors(const uint64_t *hash, const uint32_t *values, uint32_t *i
                        size_t *hllVectorSizePtr, uint16_t **hllDimRegIDCountPtr, cudaStream_t s);
 int reduceByHash(const uint64_t *hash, const uint32_t *index, const uint8_t *measures, int width, AggOp op, int n,
                  uint32_t *outIndex, uint8_t *outValues, cudaStream_t s, uint64_t *outHash = nullptr);
+// from hll_estimate.cu
+void hllEstimates(const uint8_t *vec, const uint16_t *counts, int groups, double *out, cudaStream_t s);
 
 
 // status word of the single-launch finalize / of an exchange part
@@ -2283,6 +2285,33 @@ static int64_t finalizeHLL(AggState *st, uint8_t **dimValuesPtr, uint8_t **hllVe
   return dims;
 }
 
+// HLL state -> the groups of finalizeHLL and HLL.Compute of each (hll_estimate.cu).  The register vectors stay on the
+// device and are freed here; the dim block and the estimates are allocated with deviceMalloc.
+static int64_t finalizeHLLEstimate(AggState *st, uint8_t **dimValuesPtr, double **estimatesPtr, cudaStream_t s) {
+  if (!st->hll) throw EngineError("AggStateFinalizeHLLEstimate needs a state created with AGGR_HLL");
+  if (!dimValuesPtr || !estimatesPtr) throw EngineError("null output pointer");
+  *dimValuesPtr = nullptr; *estimatesPtr = nullptr;
+  uint8_t *dims = nullptr, *vec = nullptr;
+  uint16_t *counts = nullptr;
+  size_t vecBytes = 0;
+  const int64_t g = finalizeHLL(st, &dims, &vec, &vecBytes, &counts, s);
+  if (g == 0) return 0;
+  void *est = nullptr;
+  try {
+    est = deviceAllocOrThrow(sizeof(double) * (size_t)g);
+    hllEstimates(vec, counts, (int)g, static_cast<double *>(est), s);
+    ARES_CUDA(cudaStreamSynchronize(s));
+  } catch (...) {
+    deviceFree(vec); deviceFree(counts); deviceFree(dims);
+    if (est) deviceFree(est);
+    throw;
+  }
+  deviceFree(vec); deviceFree(counts);
+  *dimValuesPtr = dims;
+  *estimatesPtr = static_cast<double *>(est);
+  return g;
+}
+
 // The dry runs: schedules `plan` for AggStates described by `specs`, without device memory.  A schedule of one launch for
 // all of them is generated and NVRTC-compiled: returns the cubin size, and *sourceOut (optional) gets a malloc'd copy of
 // the kernel's shape-specific source.  Any other schedule is reported as an error that says which kernels run instead.
@@ -2485,6 +2514,12 @@ CGoCallResHandle AggStateFinalizeHLL(void *state, uint8_t **dimValuesPtr, uint8_
   return guarded("AggStateFinalizeHLL", device, [&]() -> int64_t {
     return finalizeHLL(asState(state), dimValuesPtr, hllVectorPtr, hllVectorSizePtr, hllDimRegIDCountPtr,
                        (cudaStream_t)cudaStream);
+  });
+}
+
+CGoCallResHandle AggStateFinalizeHLLEstimate(void *state, uint8_t **dimValuesPtr, double **estimatesPtr, void *cudaStream, int device) {
+  return guarded("AggStateFinalizeHLLEstimate", device, [&]() -> int64_t {
+    return finalizeHLLEstimate(asState(state), dimValuesPtr, estimatesPtr, (cudaStream_t)cudaStream);
   });
 }
 

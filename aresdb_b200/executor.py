@@ -23,7 +23,7 @@ import numpy as np
 from . import cabi as A
 from . import expr as E
 from .memory import Buf
-from .query import AggQuery, HLLResult, QueryResult, member_dimensions
+from .query import AggQuery, HLLEstimates, HLLResult, QueryResult, member_dimensions
 from .skipping import should_skip_batch
 
 
@@ -482,6 +482,24 @@ class FusedBatchExecutor:
         res._lease = lease   # back to the pool when the result is collected
         return res
 
+    def hll_estimates(self) -> HLLEstimates:
+        """hll queries: the groups of hll_result() with their distinct-count estimates (AggStateFinalizeHLLEstimate);
+        the register vectors never leave the device."""
+        lib, sp = self.lib, self.space
+        dims, est = C.c_void_p(), C.c_void_p()
+        g = lib.AggStateFinalizeHLLEstimate(self.state, C.byref(dims), C.byref(est), sp.stream, sp.device)
+        if g == 0:
+            return HLLEstimates(self.q, 0, np.zeros(0, np.uint8), 1, np.zeros(0, np.float64))
+        nb, o_e = self.q.row_bytes * g, (self.q.row_bytes * g + 63) // 64 * 64
+        lease = _PINNED.acquire(lib, o_e + 8 * g)
+        for ptr, off, n in ((dims.value, 0, nb), (est.value, o_e, 8 * g)):
+            lib.AsyncCopyDeviceToHost(lease.ptr + off, ptr, n, sp.stream, sp.device)
+        lib.WaitForCudaStream(sp.stream, sp.device)
+        for p in (dims, est):
+            lib.DeviceFree(p, sp.device)
+        host = lease.array   # (the result copies what it keeps: the buffer goes back to the pool with the lease)
+        return HLLEstimates(self.q, g, host[:nb], g, host[o_e:o_e + 8 * g].view(np.float64).copy())
+
     def reset(self):
         self.lib.AggStateReset(self.state, self.space.stream, self.space.device)
 
@@ -673,15 +691,16 @@ class FusedRequestExecutor:
             self.lib.ExecuteBatchPlanMulti(states, len(run), C.byref(p), self.space.stream if stream is None else stream,
                                            self.space.device)
 
-    def results(self) -> list:
+    def results(self, hll_estimates: bool = False) -> list:
         """One QueryResult per query, in request order.  The non-HLL queries are finalized together (one AggStatesFinalize
-        launch and one synchronise for those that announce at most SMALL_RESULT groups)."""
+        launch and one synchronise for those that announce at most SMALL_RESULT groups).  `hll_estimates`: an HLL query
+        gives its HLLEstimates (distinct counts computed on the device) instead of the QueryResult of its carried rows."""
         idx = [i for i, q in enumerate(self.queries) if not q.is_hll]
         done = dict(zip(idx, finalize_states([self.executors[i] for i in idx])))
         out = []
         for i, ex in enumerate(self.executors):
             if i not in done:
-                out.append(ex.result())
+                out.append(ex.hll_estimates() if hll_estimates else ex.result())
             elif isinstance(done[i], Exception):
                 raise done[i]
             else:

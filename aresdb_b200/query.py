@@ -322,6 +322,16 @@ class QueryResult:
         return out
 
 
+class HLLEstimates(QueryResult):
+    """The distinct-count estimates of an hll query: the groups of its HLLResult, in the same order, with one float64
+    estimate each in `measures` (HLL.Compute on the device, AggStateFinalizeHLLEstimate).  postprocess.nested_result
+    formats it."""
+
+    def __init__(self, query: AggQuery, groups: int, block: np.ndarray, capacity: int, estimates: np.ndarray):
+        super().__init__(query, block, capacity, np.zeros(groups * query.measure_bytes, np.uint8), groups)
+        self.measures = estimates
+
+
 HLL_REGISTERS = 1 << 14          # p = 14 (reference query/common/hll.go:786)
 HLL_DENSE_THRESHOLD = HLL_REGISTERS // 4
 

@@ -179,15 +179,16 @@ class ShardedFusedRequest:
         self.dist.all_gather_into_tensor(self._recv, self._send)
         lib.AggStatesMergeParts(merged, k, self._recv.data_ptr(), w, slot, EXCHANGE_ROWS, po, do, vo, None, 0, sp.stream, sp.device)
 
-    def finalize(self) -> list:
-        """One result per query, in request order, identical on every rank: a QueryResult, or an HLLResult for HLL queries."""
-        return [r if q.is_hll else query_result(q, *r) for q, r in zip(self.queries, self._finalize())]
+    def finalize(self, hll_estimates: bool = False) -> list:
+        """One result per query, in request order, identical on every rank: a QueryResult, or for HLL queries an HLLResult
+        (`hll_estimates`: the HLLEstimates of the merged state, computed on the device)."""
+        return [r if q.is_hll else query_result(q, *r) for q, r in zip(self.queries, self._finalize(hll_estimates))]
 
-    def _finalize(self) -> list:
+    def _finalize(self, hll_estimates: bool = False) -> list:
         """The exchange and finalize step: per query, in request order, (groups, _ResultBuffers) with the result left in
-        device memory, or the HLLResult of an HLL query."""
+        device memory, or the HLLResult (HLLEstimates) of an HLL query."""
         if self.world == 1:
-            return self._results(self.local.executors, {})
+            return self._results(self.local.executors, {}, hll_estimates)
         if self._merged_dirty:
             for i in self.fixed:   # (exchange_exact resets the states it merges into)
                 self.merged[i].reset()
@@ -206,15 +207,15 @@ class ShardedFusedRequest:
             self._keep.append(gathered)
             if not self.queries[i].is_hll:
                 done[i] = self.merged[i].finalize_into(rows)
-        return self._results(self.merged, done)
+        return self._results(self.merged, done, hll_estimates)
 
-    def _results(self, executors: list, done: dict) -> list:
+    def _results(self, executors: list, done: dict, hll_estimates: bool) -> list:
         todo = [i for i, q in enumerate(self.queries) if not q.is_hll and i not in done]
         done.update(zip(todo, finalize_states([executors[i] for i in todo])))
         out = []
         for i, q in enumerate(self.queries):
             if q.is_hll:
-                out.append(executors[i].hll_result())
+                out.append(executors[i].hll_estimates() if hll_estimates else executors[i].hll_result())
             elif isinstance(done[i], Exception):
                 raise done[i]
             else:
@@ -244,9 +245,9 @@ class ShardedFusedQuery:
         """(groups, _ResultBuffers) of the WHOLE query, identical on every rank."""
         return self.request._finalize()[0]
 
-    def finalize_hll(self):
-        """HLL queries: the HLLResult of the WHOLE query, identical on every rank."""
-        return self.request._finalize()[0]
+    def finalize_hll(self, hll_estimates: bool = False):
+        """HLL queries: the HLLResult of the WHOLE query (`hll_estimates`: its HLLEstimates), identical on every rank."""
+        return self.request._finalize(hll_estimates)[0]
 
     def close(self):
         self.request.close()

@@ -313,6 +313,15 @@ CGoCallResHandle AggStateFinalizeHLL(void *state, uint8_t **dimValuesPtr, uint8_
                                      size_t *hllVectorSizePtr, uint16_t **hllDimRegIDCountPtr,
                                      void *cudaStream, int device);
 
+/* AGGR_HLL states: the distinct-count estimate of every group, computed on the device.  res = number of groups g: the
+ * groups of AggStateFinalizeHLL, in its order, with its *dimValuesPtr block (VectorCapacity g).  *estimatesPtr = g
+ * float64 values, each equal bit for bit to the reference's HLL.Compute (query/common/hll.go:735-775) of that group's
+ * register vector: bias correction up to 5m, linear counting up to 15500, truncated toward zero.  The register vectors
+ * stay on the device and are freed by the call.  Both outputs are allocated with deviceMalloc; the caller frees them
+ * with DeviceFree.  A state that is not AGGR_HLL and a null output pointer are errors.  Synchronises. */
+CGoCallResHandle AggStateFinalizeHLLEstimate(void *state, uint8_t **dimValuesPtr, double **estimatesPtr, void *cudaStream,
+                                             int device);
+
 /* Zone-map production: out[i] = min / max of the VALID values of columns[i] (at most 16 per call; Bool / 1- / 2- /
  * 4-byte integer and Float32 columns in modes 0-3; everything else, columns without a valid value, and columns whose
  * values the ColumnRange contract cannot describe — negative, >= 2^31, negative or non-finite floats — get Known = 0).
