@@ -8,8 +8,8 @@
 //                  4-cell stash bucket behind the last bucket.  RecordID {0, 0} = not found (also for a NULL key).
 //   foreignLoad    value of a foreign column at a RecordID (reference RecordIDJoinIterator::dereference,
 //                  query/iterator.hpp:846-931): batch = batchID - baseBatchID, bounds check against the last batch's
-//                  record count, mode-0 batches yield the column default, then the optional enum -> timezone-offset
-//                  table; an unmatched row is (unspecified, NULL) — 0 here.
+//                  record count, mode-0 batches yield the column default (not mapped), the others go through the
+//                  optional enum -> timezone-offset table; an unmatched row is (unspecified, NULL) — 0 here.
 #pragma once
 #include "column.cuh"
 #include "murmur.cuh"
@@ -88,8 +88,9 @@ __device__ __forceinline__ Cell foreignLoad(const ForeignDesc &F, unsigned long 
   if (b < 0 || b >= F.numBatches || b >= kMaxForeignBatches) return c;   // (the reference would read out of bounds)
   const InputDesc &d = F.batches[b];
   c = loadInput(d, index, nullptr, nullptr, 0, hi);
-  if (F.tzLookup != nullptr && d.vclass != VC_UUID && d.vclass != VC_I64) {
-    // an enum column mapped through the timezone table: (table[enum], valid), 0 beyond the table
+  if (F.tzLookup != nullptr && d.mode != 0 && d.vclass != VC_UUID && d.vclass != VC_I64) {
+    // an enum column mapped through the timezone table: (table[enum], valid), 0 beyond the table; a mode-0 batch yields
+    // the column default as it is (the reference returns its constant iterator before the lookup)
     const int32_t e = d.vclass == VC_F32 ? (int32_t)__uint_as_float((uint32_t)c.v) : (int32_t)(uint32_t)c.v;
     const int32_t off = e >= 0 && e < F.tzSize ? (int32_t)F.tzLookup[e] : 0;
     c.v = d.vclass == VC_F32 ? (uint64_t)__float_as_uint((float)off) : d.vclass == VC_BOOL ? (uint64_t)(off != 0) : (uint64_t)(uint32_t)off;

@@ -250,14 +250,17 @@ static int read_input(const InputVector *in, uint32_t i, const uint32_t *index,
       RecordID rid = f->RecordIDs[i];
       out->k = k;
       out->valid = false;
-      if (rid.batchID && (rid.batchID - f->BaseBatchID < f->NumBatches - 1 || rid.index < (uint32_t)f->NumRecordsInLastBatch)) {
-        VectorPartySlice vp = f->Batches[rid.batchID - f->BaseBatchID];
+      /* (a batch outside [0, NumBatches) and a negative enum are NULL and offset 0 here, where the reference reads out
+       * of bounds; the engine does the same, join.cuh foreignLoad) */
+      const int32_t b = rid.batchID - f->BaseBatchID;
+      if (rid.batchID && (b < f->NumBatches - 1 || rid.index < (uint32_t)f->NumRecordsInLastBatch) && b >= 0 && b < f->NumBatches) {
+        VectorPartySlice vp = f->Batches[b];
         vp.DataType = f->DataType;
         if (vp.BasePtr == NULL) vp.DefaultValue = f->DefaultValue;
         *out = read_vp(&vp, rid.index, NULL, 0);
-        if (f->TimezoneLookup && k != K_UUID && k != K_I64) {
+        if (f->TimezoneLookup && f->Batches[b].BasePtr != NULL && k != K_UUID && k != K_I64) {   /* mode 0: not mapped */
           int e = k == K_F32 ? (int)out->v.f : k == K_BOOL ? (int)out->v.b : (int)out->v.u;
-          int16_t off = e < f->TimezoneLookupSize ? f->TimezoneLookup[e] : 0;
+          int16_t off = e >= 0 && e < f->TimezoneLookupSize ? f->TimezoneLookup[e] : 0;
           if (k == K_F32) out->v.f = (float)off; else if (k == K_BOOL) out->v.b = off != 0; else out->v.u = (uint32_t)(int32_t)off;
         }
       }

@@ -13,12 +13,12 @@ def _rotl32(x, r):
     return ((x << np.uint64(r)) | (x >> np.uint64(32 - r))) & M32
 
 
-def murmur3_32(rows: np.ndarray) -> np.ndarray:
-    """rows: uint8[n, len] -> uint32[n] (seed 0)."""
+def murmur3_32(rows: np.ndarray, seed: int = 0) -> np.ndarray:
+    """rows: uint8[n, len] -> uint32[n]."""
     n, ln = rows.shape
     rows = np.ascontiguousarray(rows)
     words = np.ascontiguousarray(rows[:, :ln // 4 * 4]).view("<u4").reshape(n, ln // 4).astype(np.uint64)
-    h = np.zeros(n, np.uint64)
+    h = np.full(n, seed & 0xFFFFFFFF, np.uint64)
     for i in range(ln // 4):
         k = (words[:, i] * np.uint64(0xcc9e2d51)) & M32
         k = _rotl32(k, 15)

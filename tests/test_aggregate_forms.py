@@ -239,7 +239,10 @@ def _cls(dt):
 
 
 def packed_rows(hb, dims):
-    """uint8[n, rowBytes]: dimension values in layout order (widest first), then one validity byte each."""
+    """uint8[n, rowBytes]: dimension values in layout order (widest first), then one validity byte each.  dims=None:
+    the rows the caller packed into hb["packed"]."""
+    if dims is None:
+        return hb["packed"]
     n = hb["rows"]
     w = hb["w"].astype("<u2").view(np.uint8).reshape(n, 2)
     one = np.ones((n, 1), np.uint8)
@@ -271,9 +274,9 @@ def restate(hbs, kind, dt, dims="kw", filters=(BASE_FILTER,), mode=A.ARES_REDUCE
     rows = np.vstack(keys)
     v, ok, mult = np.concatenate(vals), np.concatenate(oks), np.concatenate(mult).astype(np.int64)
     if mode == A.ARES_REDUCE_SORT:
-        key = np.zeros(len(rows), np.uint64)
-        for b in range(rows.shape[1]):
-            key |= rows[:, b].astype(np.uint64) << np.uint64(8 * b)
+        # the row's bytes are its identity (as one void scalar: rows may be longer than 8 bytes)
+        key = np.ascontiguousarray(rows).view(np.dtype((np.void, rows.shape[1]))).reshape(-1) if rows.shape[1] else \
+            np.zeros(len(rows), np.uint64)
     else:
         key = hashes.murmur3_32(rows)
     uniq, first, inv = np.unique(key, return_index=True, return_inverse=True)
