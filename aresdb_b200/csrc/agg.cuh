@@ -45,6 +45,8 @@ __device__ __forceinline__ uint64_t rollingAvg(uint64_t lhs, uint64_t rhs) {
   return ((uint64_t)total << 32) | __float_as_uint(res);
 }
 
+// Float MIN / MAX keep a NaN once one is folded in: the value of a group whose rows are NaN is NaN, as the reference's
+// Reduce gives it, whatever neutral element the accumulator started from (an ordered compare alone never lets a NaN in).
 __device__ __forceinline__ uint64_t aggCombine(AggOp op, uint64_t a, uint64_t b) {
   switch (op) {
     case OP_SUM_I32: return (uint32_t)((uint32_t)a + (uint32_t)b);
@@ -53,10 +55,16 @@ __device__ __forceinline__ uint64_t aggCombine(AggOp op, uint64_t a, uint64_t b)
     case OP_SUM_F64: return (uint64_t)__double_as_longlong(__dadd_rn(__longlong_as_double((long long)a), __longlong_as_double((long long)b)));
     case OP_MIN_U32: return (uint32_t)b < (uint32_t)a ? (uint32_t)b : (uint32_t)a;
     case OP_MIN_I32: return (int32_t)(uint32_t)b < (int32_t)(uint32_t)a ? (uint32_t)b : (uint32_t)a;
-    case OP_MIN_F32: return __uint_as_float((uint32_t)b) < __uint_as_float((uint32_t)a) ? (uint32_t)b : (uint32_t)a;
+    case OP_MIN_F32: {
+      const float x = __uint_as_float((uint32_t)a), y = __uint_as_float((uint32_t)b);
+      return (y < x || (y != y && x == x)) ? (uint32_t)b : (uint32_t)a;
+    }
     case OP_MAX_U32: return (uint32_t)a < (uint32_t)b ? (uint32_t)b : (uint32_t)a;
     case OP_MAX_I32: return (int32_t)(uint32_t)a < (int32_t)(uint32_t)b ? (uint32_t)b : (uint32_t)a;
-    case OP_MAX_F32: return __uint_as_float((uint32_t)a) < __uint_as_float((uint32_t)b) ? (uint32_t)b : (uint32_t)a;
+    case OP_MAX_F32: {
+      const float x = __uint_as_float((uint32_t)a), y = __uint_as_float((uint32_t)b);
+      return (x < y || (y != y && x == x)) ? (uint32_t)b : (uint32_t)a;
+    }
     default: return rollingAvg(a, b);
   }
 }

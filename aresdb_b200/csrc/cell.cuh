@@ -256,6 +256,17 @@ ARES_HD Cell evalUnary(int fn, Cell a, ValClass ic, ValClass *rc) {
 }
 
 // ---- binary functors ------------------------------------------------------------------
+// Float32 Plus / Minus / Multiply / Divide, each rounded once to nearest-even: what the reference's per-node calls (every
+// functor writes a float vector) and x86 compute.  On the device the _rn intrinsics keep the compiler from contracting
+// `a * b` and a following `+ c` / `- c` of the same row into one FFMA (NVRTC compiles with --fmad=true).
+ARES_HD float f32Arith(int fn, float x, float y) {
+#ifdef __CUDA_ARCH__
+  return fn == Plus ? __fadd_rn(x, y) : fn == Minus ? __fsub_rn(x, y) : fn == Multiply ? __fmul_rn(x, y) : __fdiv_rn(x, y);
+#else
+  return fn == Plus ? x + y : fn == Minus ? x - y : fn == Multiply ? x * y : x / y;
+#endif
+}
+
 // Both operands are already converted to the common class `tc` (VC_I32, VC_U32 or VC_F32).
 ARES_HD Cell evalBinary(int fn, Cell a, Cell b, ValClass tc, ValClass *rc) {
   Cell r; r.v = 0; r.valid = false;
@@ -300,9 +311,7 @@ ARES_HD Cell evalBinary(int fn, Cell a, Cell b, ValClass tc, ValClass *rc) {
     if (!a.valid || !b.valid) return r;
     r.valid = true;
     if (isFloat) {
-      float x = asF32(a.v), y = asF32(b.v), z;
-      z = fn == Plus ? x + y : fn == Minus ? x - y : fn == Multiply ? x * y : x / y;
-      r.v = fromF32(z);
+      r.v = fromF32(f32Arith(fn, asF32(a.v), asF32(b.v)));
     } else if (tc == VC_I32) {
       int32_t x = (int32_t)(uint32_t)a.v, y = (int32_t)(uint32_t)b.v; uint32_t z;
       switch (fn) {
@@ -340,20 +349,25 @@ ARES_HD Cell evalBinary(int fn, Cell a, Cell b, ValClass tc, ValClass *rc) {
   return a;
 }
 
-// Identity element of an aggregate in the sink's value class
-// (reference query/utils.hpp:169-184: note MAX_FLOAT uses FLT_MIN, the smallest positive
-// normal, not -FLT_MAX; reproduced as is).
 // SUM measures of an RLE batch count `count` times: value * count in the sink's arithmetic
-// (reference query/iterator.hpp:626-645, 704-709).
+// (reference query/iterator.hpp:626-645, 704-709).  The float products are rounded on their own: never contracted with
+// the accumulation that follows.
 ARES_HD uint64_t mulCount(uint64_t v, ValClass oc, uint32_t count) {
   switch (oc) {
     case VC_I32: case VC_U32: return (uint32_t)((uint32_t)v * count);
-    case VC_F32: return fromF32(asF32(v) * (float)count);
+    case VC_F32: return fromF32(f32Arith(Multiply, asF32(v), (float)count));
     case VC_I64: return (uint64_t)((int64_t)v * (int64_t)(uint64_t)count);
+#ifdef __CUDA_ARCH__
+    default: return fromF64(__dmul_rn(asF64(v), (double)count));
+#else
     default: return fromF64(asF64(v) * (double)count);
+#endif
   }
 }
 
+// Identity element of an aggregate in the sink's value class
+// (reference query/utils.hpp:169-184: note MAX_FLOAT uses FLT_MIN, the smallest positive
+// normal, not -FLT_MAX; reproduced as is).
 ARES_HD uint64_t aggIdentity(int aggFunc, ValClass oc) {
   double d = 0; int64_t s = 0; bool isS = false, isD = false; uint64_t u = 0;
   switch (aggFunc) {
