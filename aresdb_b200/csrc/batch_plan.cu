@@ -1233,7 +1233,7 @@ static bool memberSlots(DevPlan &P, size_t avail) {
       if ((M.dims >> j) & 1u) total *= (uint64_t)P.denseCnt[j] + 1;
     if (total > kDenseMaxSlots) return false;
     M.total = (uint32_t)total;
-    sb[m] = M.denseFx ? 12 : 9;
+    sb[m] = denseSlotBytes(M.denseFx);
     r16[m] = (total + 15) / 16 * 16;
     need += r16[m] * sb[m];
   }
@@ -1299,11 +1299,10 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
           }
           continue;
         }
-        // three 32-bit piece counters, or flag + 8-byte accumulator; HLL: one 32-bit map entry (slot -> group's registers)
-        size_t slotBytes = P.hll ? 4 : P.denseFx ? 12 : 9;
+        size_t slotBytes = denseSlotBytes(P.denseFx, P.hll);
         if (P.nmeas > 1) {
           slotBytes = 0;
-          for (int m = 0; m < P.nmeas; m++) slotBytes += P.meas[m].denseFx ? 12 : 9;
+          for (int m = 0; m < P.nmeas; m++) slotBytes += denseSlotBytes(P.meas[m].denseFx);
         }
         uint32_t cap = (uint32_t)((budget - need) / slotBytes / 16 * 16);
         if (cap > kDenseMaxSlots) cap = kDenseMaxSlots;
@@ -1371,11 +1370,10 @@ static size_t layoutStages(DevPlan &P, uint32_t expectedGroups) {
   P.numFullTiles = fullTiles(tileRows);
   P.stageBytes = (uint32_t)stageBytes;
   P.smemSlots = slots;
-  P.tableBytes = P.denseNd != 0 ? (slots * (P.hll ? 4 : P.denseFx ? 12 : 9) + 127) / 128 * 128 : slots * 8;
+  P.tableBytes = P.denseNd != 0 ? (slots * denseSlotBytes(P.denseFx, P.hll) + 127) / 128 * 128 : slots * 8;
   if (P.nmeas > 1) {
     P.tableBytes = 0;
-    for (int m = 0; m < P.nmeas; m++)
-      P.tableBytes += ((P.memberDims ? P.meas[m].slots : slots) * (P.meas[m].denseFx ? 12 : 9) + 127) / 128 * 128;
+    for (int m = 0; m < P.nmeas; m++) P.tableBytes += measureRegionBytes(P, m);
   } else {
     describeMeasure(P, P.meas[0]);
   }

@@ -147,6 +147,16 @@ inline bool positiveLiteralSum(const DevInst &I, uint8_t aggOp) {
          I.akind == OPK_CONST && I.avalid && (I.aclass == VC_I32 || I.aclass == VC_U32) && (int32_t)I.aconst > 0;
 }
 
+// Bytes of one direct-indexed slot in the CTA: three 32-bit piece counters (exact-integer float sum, `fx`) or a "reached"
+// flag and an 8-byte accumulator; HLL: one 32-bit map entry (slot -> the group's registers)
+inline uint32_t denseSlotBytes(bool fx, bool hll = false) { return hll ? 4u : fx ? 12u : 9u; }
+
+// Measure m's region of the table area of a multi-measure plan (the regions follow the 128-byte header in measure order):
+// its slots (member dimensions: its own, else the plan's), 128-byte aligned
+inline uint32_t measureRegionBytes(const DevPlan &P, int m) {
+  return ((P.memberDims ? P.meas[m].slots : P.smemSlots) * denseSlotBytes(P.meas[m].denseFx) + 127u) / 128u * 128u;
+}
+
 constexpr uint32_t kDenseMaxSlots = 8192;   // = slots of a CTA's accumulator slice in AggState::ctaAcc
 constexpr uint32_t kFxMaxRowsPerCta = 1u << 21;   // each 32-bit piece accumulator takes 2^21 adds of an 11-bit piece
 constexpr uint32_t kGlobalDenseMaxSlots = 1u << 21;   // 16 MB of accumulators per state, allocated on first use
